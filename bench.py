@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - S2ST utterances/sec for seamlessM4T_v2_large + vocoder_v2 on B200 (BASELINE.json metric).
+"""bench.py - S2ST utterances/sec for seamlessM4T_v2_large + vocoder_v2 on H100 (BASELINE.json metric).
 
 A "step" is one pass of the whole hot path (fbank -> Conformer encoder -> beam-search text decoder -> NAR T2U ->
 Code-HiFiGAN) over one batch of 32 x 10 s synthetic 16 kHz utterances per GPU through `Translator.predict`, with
@@ -20,6 +20,9 @@ random-init weights of the named architecture (no checkpoints are reachable offl
   --config s2tt    : BASELINE configs[1] (8 x 10 s, encoder + text decoder only).
   --config stream  : BASELINE configs[4] (SeamlessStreaming EMMA S2ST, one 30 s synthetic stream in 320 ms segments): compute
                      latency per source segment and the real-time factor.
+  --dump-outputs DIR : after the timed steps, what the last timed step returned to its caller, as DIR/<name>.npy (texts as
+                     unicode code points, unit ids, waveforms; padded with -1 / 0, lengths alongside).  Inputs and weights
+                     are seeded, so two builds can be compared output for output.
 """
 import argparse
 import ctypes
@@ -59,7 +62,8 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sustained=d["bf16_tflops_sustained"], src="MEASURED_PEAKS.json")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sustained=1400.0, src="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense fp16 / bf16 - not measured figures
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sustained=989.0, src="H100 SXM data sheet (dense fp16, 700 W)")
 
 
 class ClockSampler:
@@ -215,7 +219,7 @@ def cpu_baseline_block(task, batch, timed_runs, warmup=True, trace=None):
 def workload_config(cfg, batch, world):
     """`config` of the bench line: the workload only, identical in both arms (how this arm runs it is under `pipeline`)."""
     return {"workload": cfg["workload"], "per_gpu_batch": batch, "global_batch": batch * world, "parallelism": f"dp{world}",
-            "l2": "working set (3.5 GB fp16 weights + activations) >> 126 MB L2, no explicit flush",
+            "l2": "working set (3.5 GB fp16 weights + activations) >> 50 MB L2, no explicit flush",
             "weights": "random-init, seeded", "accumulate": "f32"}
 
 
@@ -223,7 +227,7 @@ def run_reference(args, rank):
     if rank != 0:
         return
     cfg = CONFIGS[args.config]
-    block, _ = cpu_baseline_block(cfg["task"], 4, max(1, min(args.steps, 3)), warmup=args.warmup > 0)
+    block, _ = cpu_baseline_block(cfg["task"], 4, args.steps, warmup=args.warmup > 0)
     v = block["value"]
     line = {"impl": "reference", "metric": cfg["metric"], "value": v, "unit": "utt/s", "n_gpus": args.gpus,
             "steps": len(block["seconds_per_run"]), "warmup": 1 if args.warmup > 0 else 0,
@@ -231,7 +235,7 @@ def run_reference(args, rank):
             "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": workload_config(cfg, cfg["batch"], max(1, args.gpus)),
             "sample": "each step = batch 4 of the workload's utterances on the host CPU (BASELINE.md 3 protocol: 1 warm-up, "
-                      "at most 3 timed runs, thread count = fastest of a probe)",
+                      "--steps timed runs, thread count = fastest of a probe)",
             "cpu_baseline": block,
             "e2e": {"value": v, "unit": "utt/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     print(json.dumps(line))
@@ -302,19 +306,6 @@ def decode_step_bytes(eng, batch, steps_dec):
     kv_self = 2 * eng.cfg.dec_layers * R * eng.M * 2 * (steps_dec / 2.0)
     kv_cross = eng.cfg.dec_layers * batch * 63 * 2 * eng.M * 2
     return w_bytes + kv_self + kv_cross, dict(weights=w_bytes, kv_self_mean=kv_self, kv_cross=kv_cross)
-
-
-def measured_decode_traffic():
-    """DRAM bytes of one beam-search step from this round's ncu passes over `bench.py --profile-only` with a 13-step search
-    (tools/ncu_summary.py).  Two passes: `--cache-control none` (L2 contents carried from kernel to kernel, as in a real
-    step: split-K partials and activations stay in L2) is the figure reported as `traffic`; the default pass flushes the
-    caches before every launch, so every intermediate is counted as DRAM traffic (`traffic_cold`)."""
-    out = {}
-    for key, name in (("warm", "r02warm_decode_step_dram.json"), ("cold", "r02_decode_step_dram.json")):
-        p = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(p):
-            out[key] = json.load(open(p))
-    return out
 
 
 def stage_table(stages, batch, pk, eng, task):
@@ -400,7 +391,7 @@ def run_stream(args, device):
     mono = load_monotonic_decoder_model("base_v2", device=device, state_dict=S.make_monotonic_state_dict(cfg, seed=2), tokenizers=toks)
     wave = torch.cat([w for w in S.make_waveforms(3, SAMPLES, seed=4321)])  # 30 s
     results = []
-    for rep in range(max(1, args.warmup) + max(1, min(args.steps, 3))):
+    for rep in range(max(1, args.warmup) + args.steps):
         st = StreamingS2ST(tr.model, mono, tr.vocoder, TGT_LANG)
         torch.cuda.synchronize()
         ids, chunks = st.run(wave)
@@ -424,6 +415,30 @@ def run_stream(args, device):
     print(json.dumps(line))
 
 
+def dump_outputs(out_dir, texts, speech):
+    """What Translator.predict returned for the batch, as float arrays: texts as unicode code points (-1 padded), unit ids
+    (-1 padded) and waveforms (float32, 0 padded), each with its per-utterance lengths."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+
+    def padded(rows, fill, dtype):
+        n = max((len(r) for r in rows), default=0)
+        a = np.full((len(rows), n), fill, dtype=dtype)
+        for i, r in enumerate(rows):
+            a[i, :len(r)] = r
+        return a, np.array([len(r) for r in rows], dtype=np.float64)
+
+    arrays = {}
+    arrays["text_codepoints"], arrays["text_lens"] = padded([[ord(c) for c in t] for t in texts], -1, np.float64)
+    if speech is not None:
+        arrays["units"], arrays["unit_lens"] = padded(speech.units, -1, np.float64)
+        wavs = [w.float().flatten().cpu().numpy() for w in speech.audio_wavs]
+        arrays["audio"], arrays["audio_lens"] = padded(wavs, 0.0, np.float32)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -435,7 +450,13 @@ def main():
     ap.add_argument("--profile-only", action="store_true", help="one device-resident step only (for ncu launch lists)")
     ap.add_argument("--lanes", type=int, default=int(os.environ.get("SB_LANES", "4")),
                     help="batches in flight per GPU (parallel.LanePool: one host thread + stream + search state each); 1 = serial")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (texts, units, waveforms) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and (args.impl == "reference" or args.config == "stream" or args.profile_only):
+        ap.error("--dump-outputs applies to the timed GPU path of --config s2st / s2tt only")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -498,15 +519,18 @@ def main():
     main_stream = torch.cuda.current_stream()
 
     def run_device_steps(n):
-        """n steps, each one batch through the whole path; with lanes, LANES of them are in flight at any time."""
+        """n steps, each one batch through the whole path; with lanes, LANES of them are in flight at any time.
+        Returns what the last step returned."""
+        out = None
         if pool is None:
             for _ in range(n):
-                step_device()
-            return
+                out = step_device()
+            return out
         futs = [pool.submit(i, step_device) for i in range(n)]
         for f in futs:
-            _, done = f.result()
+            out, done = f.result()
             main_stream.wait_event(done)
+        return out
 
     # ---- device-resident leg
     if pool is not None:
@@ -518,10 +542,12 @@ def main():
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     torch.cuda.synchronize()
     e0.record()
-    run_device_steps(args.steps)
+    last_out = run_device_steps(args.steps)
     e1.record()
     sync_all()
     ms_dev = max_over_ranks(e0.elapsed_time(e1) / args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *last_out)
     launches_total = launches_now() - n0  # kernels of this library launched inside the timed region (graph replays included)
     launches = launches_total // args.steps
     clocks = sampler.stop() if sampler else None
@@ -621,21 +647,10 @@ def main():
             line["stages_ms"] = stages
             line["stages"] = tab
             bs = tab["beam_search"]
-            tm = measured_decode_traffic() if task == "s2st" else {}
-            tsel = tm.get("warm") or tm.get("cold")
-            traffic = tsel["dram_bytes_per_step"] if tsel else None
-            tsrc = None
-            if tsel:
-                alg_prof, _ = decode_step_bytes(eng, BATCH, tsel["steps_profiled"])
-                tsrc = (f"ncu dram__bytes_read.sum + dram__bytes_write.sum over the launches of a {tsel['steps_profiled']}-step search, per step "
-                        f"({'--cache-control none' if 'warm' in tm else 'caches flushed per launch'}; profiles/r02warm_kernels_ncu.txt, "
-                        f"profiles/r02_kernels_ncu.txt); algorithmic bytes at those positions: {alg_prof / 1e9:.2f} GB + 0.16 GB of fp32 "
-                        f"logits the step also writes; the search's K/V reads grow with the position")
             line["roofline"] = {"bound": "hbm", "kernel": "one beam-search step = decoder-step kernels + vocabulary projection + top-K "
                                                           f"({bs['steps']} steps, {100 * bs['ms'] / ms_serial:.0f} % of a batch's time)",
                                 "achieved": bs["achieved_gbs"], "peak": pk["hbm"], "unit": "GB/s", "frac": bs["frac"],
-                                "traffic": traffic, "traffic_cold": (tm.get("cold") or {}).get("dram_bytes_per_step"),
-                                "traffic_source": tsrc, "algorithmic_bytes": bs["algorithmic_bytes_per_step"],
+                                "algorithmic_bytes": bs["algorithmic_bytes_per_step"],
                                 "ms_per_launch_group": bs["ms_per_step"], "peak_source": pk["src"], "in_flight": 1}
             if pool is not None:
                 # how the step actually runs: LANES searches interleaved on the device.  Every lane's step still needs every

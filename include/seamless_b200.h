@@ -1,5 +1,5 @@
 /*
- * seamless_b200.h - C ABI of the B200-native SeamlessM4T-v2 S2ST hot path.
+ * seamless_b200.h - C ABI of the H100-native SeamlessM4T-v2 S2ST hot path.
  *
  * Convention (SURVEY.md 8b): one `extern "C" int sb_<op>(...)` per module of the path, plain device pointers and
  * sizes, a CUDA stream, an int return code (0 = ok, otherwise a negative SB_E* code; sb_last_error() gives text).
@@ -39,7 +39,7 @@ int sb_version(void);
 int64_t sb_launch_count(void);
 
 /* ------------------------------------------------------------------------------------------------------------------
- * sb_gemm - fused Linear / Conv1d-as-GEMM on tcgen05 tensor cores (TMA -> smem -> tcgen05.mma -> TMEM -> epilogue).
+ * sb_gemm - fused Linear / Conv1d-as-GEMM on Hopper tensor cores (TMA -> smem -> wgmma -> registers -> epilogue).
  *   acc[m, n] = sum_{tap, c} A[a_row0 + m + tap*dil, c] * W[n, tap*c_in + c]
  *   v   = act(acc + bias[n])            (glu: v[j] = (acc[2j]+b[2j]) * sigmoid(acc[2j+1]+b[2j+1]), N/2 outputs)
  *   out[q, n] = gamma * (alpha * v + res1[q, n] + res2[q, n]),  q = m + out_row0
@@ -87,13 +87,13 @@ int sb_gemm(const sb_gemm_t* g, sb_stream_t stream);
  * the TMA-store epilogue).  Only a/w/shape fields of `g` are used. */
 int sb_gemm_splitk(const sb_gemm_t* g, int32_t splits, float* partials, int64_t slice_rows, sb_stream_t stream);
 /* The same products for at most 160 rows (one decoder step of 32 sentences x beam 5) on a short-latency kernel
- * (cp.async + mma.sync, skinny_gemm.cu) instead of the TMA/tcgen05 pipeline, whose fixed set-up cost dominates at this
+ * (cp.async + mma.sync, skinny_gemm.cu) instead of the TMA/wgmma pipeline, whose fixed set-up cost dominates at this
  * size.  partials != NULL: split-K mode, same output contract as sb_gemm_splitk.  partials == NULL (splits must be 1):
  * out = act(a . w^T + bias) in fp16, act in {none, relu}.  sb_gemm_skinny_supported returns 1 when the shape qualifies
  * (taps 1, m <= 160, n % 64 == 0, c_in % (64 * splits) == 0, 16-byte aligned operands). */
 int sb_gemm_skinny_supported(const sb_gemm_t* g, int32_t splits);
 int sb_gemm_skinny(const sb_gemm_t* g, int32_t splits, float* partials, int64_t slice_rows, sb_stream_t stream);
-/* The same products for at most 256 rows in TRANSPOSED form on tcgen05 (decode_gemm.cu): a 128-feature weight tile is the
+/* The same products for at most 256 rows in TRANSPOSED form on wgmma (decode_gemm.cu): a 128-feature weight tile is the
  * MMA A operand and all rows are the B operand, so a CTA reads its weights once and the activations once per k-block
  * (the row-major kernel re-reads a 128-row activation tile for every 64 features and is L2 -> SM bound at 160 rows).
  * partials != NULL: split-K mode, same output contract as sb_gemm_splitk (splits need not divide the k-blocks).

@@ -155,5 +155,5 @@ def require_cuda():
     import torch
 
     if not torch.cuda.is_available():
-        raise RuntimeError("seamless_communication_b200 needs a CUDA device (sm_100a); there is no CPU fallback.")
+        raise RuntimeError("seamless_communication_b200 needs a CUDA device (sm_90a); there is no CPU fallback.")
     return load()

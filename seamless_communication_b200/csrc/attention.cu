@@ -1,7 +1,7 @@
 // sb_attention: flash-style multi-head attention, head_dim 64, fp16 in/out, fp32 softmax & accumulation.
 //
 // One CTA = 64 query rows of one (batch, head); 4 warps x 16 rows; key/value blocks of 64 staged in shared memory.
-// Tensor-core math uses mma.sync.m16n8k16 (attention is ~4 % of the encoder FLOPs; the GEMMs around it are tcgen05).
+// Tensor-core math uses mma.sync.m16n8k16 (attention is ~4 % of the encoder FLOPs; the GEMMs around it are wgmma).
 // Shaw relative-position bias (models/conformer_shaw/builder.py:127-146): instead of the reference's (S,S,64) gather
 // + einsum, each warp computes QR = q . rel_k^T once (16 x 73, a tiny GEMM) and the score tile adds
 // QR[i, clamp(j-i,-L,R)+L] by a shared-memory lookup.
@@ -511,9 +511,9 @@ extern "C" int sb_attention(const void* q, int64_t q_ld, const void* k, int64_t 
   a.batch = batch; a.heads = heads; a.sq = sq; a.sk = sk; a.q_rows = q_rows; a.q_halo = q_halo;
   a.kv_rows = kv_rows; a.kv_halo = kv_halo; a.kv_lens = kv_lens; a.causal = causal;
   a.rel_k = (const elem_t*)rel_k; a.rel_left = rel_left; a.rel_right = rel_right;
-  // opt-in: measured on B200 at the encoder shape (tools/attn_bench.py) the 128-row kernel is SLOWER, 457 vs 316 us per
-  // launch: 242 registers and 108 KB leave 8 warps per SM against 12, and with one warp doing QK^T -> softmax -> PV in turn
-  // the tensor pipe idles during the softmax unless other warps fill in; shared-memory bandwidth was not the limit
+  // opt-in (not timed on H100; tools/attn_bench.py compares the two): the 128-row kernel needs 244 registers per thread in
+  // the sm_90a build and 108 KB of shared memory, so fewer warps share an SM, and with one warp doing QK^T -> softmax -> PV
+  // in turn the tensor pipe idles during the softmax unless other warps fill in
   static int v2 = -1;
   if (v2 < 0) { const char* e = getenv("SB_ATTENTION_V2"); v2 = (e != nullptr && atoi(e) != 0) ? 1 : 0; }
   if (v2) {

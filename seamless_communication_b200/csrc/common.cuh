@@ -1,4 +1,4 @@
-// Shared device/host helpers for the sm_100a kernels.
+// Shared device/host helpers for the sm_90a kernels.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -48,15 +48,16 @@ inline void count_launch(int n = 1) { __atomic_fetch_add(&g_launch_count, (long 
 
 // Programmatic dependent launch (PDL, opt-in with SB_PDL=1): every kernel waits for its prerequisites right before it
 // first touches data produced upstream and only THEN lets its own dependents launch, so launch latency, prologues
-// (barrier init, TMEM allocation, descriptor fetch) and - in the GEMMs - the weight loads of kernel N+1 overlap with
-// kernel N, while at most one generation of dependents is resident.  (Round 1 triggered at kernel entry: the whole
-// chain then launches ahead, every waiting kernel pins shared memory / TMEM, and the step got slower - 425 vs 402 ms.)
+// (barrier init, descriptor fetch) and - in the GEMMs - the weight loads of kernel N+1 overlap with
+// kernel N, while at most one generation of dependents is resident.  (Triggering at kernel entry instead would let the
+// whole chain launch ahead, with every waiting kernel pinning shared memory.)
 // Both instructions are no-ops when the kernel was launched without the attribute.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_sync() { pdl_wait(); pdl_trigger(); }
 
 bool pdl_enabled();
+int sm_count();  // SMs of the current device (cached per device)
 
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {

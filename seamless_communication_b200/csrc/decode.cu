@@ -125,7 +125,7 @@ __device__ __forceinline__ void attend_one(const elem_t* __restrict__ qp, int nk
 __device__ __forceinline__ void gather_head_vec(const float* __restrict__ part, int splits, long long slice_rows, long long ld,
                                                 const float* __restrict__ bias, long long row, int col0, elem_t* dst) {
   // All slices are requested before the first one is used (a plain loop serialises one L2 round trip per slice: with 4-8
-  // slices that was most of the attention kernels' time, profiles/r02_notes.md).
+  // slices that was most of the attention kernels' time).
   const int lane = threadIdx.x & 31;
   float2 acc = *reinterpret_cast<const float2*>(bias + col0 + 2 * lane);
   const float* pp = part + row * ld + col0 + 2 * lane;
@@ -200,8 +200,8 @@ __global__ void __launch_bounds__(128) decode_self_attn_kernel(const elem_t* __r
   attend_one(qp, step + 1, kptr, vptr, sc, out + (long long)r * dim + hoff);
 }
 
-// Same computation with the dependent round trips removed (a kernel of this size costs ~1 us per DEPENDENT global access,
-// and the version above chains 13 of them: step, three slice gathers, ancestry, four key rounds, four value rounds):
+// Same computation with the dependent round trips removed (a kernel of this size pays a full L2 / HBM latency per
+// DEPENDENT global access, and the version above chains 13 of them: step, three slice gathers, ancestry, four key rounds, four value rounds):
 //   round 1: step index, every split-K slice of q | k | v, the whole ancestry row - all independent, requested together;
 //   then 32 keys per round with the key AND the value rows of the round in flight together (online softmax).
 __global__ void __launch_bounds__(128) decode_self_attn2_kernel(const float* __restrict__ part, int splits, long long slice_rows,
@@ -364,7 +364,7 @@ __global__ void __launch_bounds__(128) decode_cross_attn_kernel(const elem_t* __
 // Cross-attention of ALL hypotheses of one sentence in one CTA (grid: sentence x head, one warp per hypothesis).  The beams
 // of a sentence attend the same encoder keys: the CTA stages K and V of its (sentence, head) in shared memory once instead
 // of every (row, head) warp streaming them from L2 (160 rows x 16 heads x 63 keys x 256 B = 41 MB per layer and step against
-// 8 MB unique; measured 10.0 us per launch for the per-row kernel).  Scores -> probabilities (shared memory) -> values:
+// 8 MB unique).  Scores -> probabilities (shared memory) -> values:
 // no dependent global round trip after the staging.  Lane = (key group kg, dim chunk dc) as in attend_one.
 __global__ void __launch_bounds__(256) decode_cross_attn_shared_kernel(const float* __restrict__ part, int splits, long long slice_rows,
                                                                        const float* __restrict__ bias, const elem_t* __restrict__ k,

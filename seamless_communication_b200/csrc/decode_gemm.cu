@@ -1,12 +1,10 @@
 // sb_gemm_decode: the decoder-step products at <= 256 rows (one beam-search step: 160 rows) in "transposed" form.
 //
 // At 160 rows the general kernel (gemm_tcgen05.cu: rows = MMA M, 64 output features per CTA) is bound by L2 -> SM traffic, not
-// by HBM: every CTA re-reads its 128-row activation tile for each of its few weight rows - the FFN inner product moves
-// 128 x 2 CTAs x (256 KB activations + 128 KB weights) = 98 MB through L2 for 16 MB of weights (10.7 us per launch,
-// profiles/r02_notes.md).  Here a 128-FEATURE weight tile is the tcgen05 A operand and ALL rows are the B operand (N = rows
-// padded to 16, one TMEM accumulator): a CTA reads its weight tile once and the activations once per k-block, 36 KB per
-// k-block for 128 x 160 outputs - 37 MB for the same product.  One (tile, K-slice) unit per CTA, a deep TMA ring (the unit
-// is a chain of k-blocks), one producer warp, one MMA warp, four epilogue warps (TMEM lane = output feature).
+// by HBM: every CTA re-reads its 128-row activation tile for each of its few weight rows.  Here a 128-FEATURE weight tile is
+// the wgmma A operand (two consumer warpgroups, 64 features each) and ALL rows are the B operand (N = rows padded to a
+// power of two >= 32, fp32 accumulators in registers): a CTA reads its weight tile once and the activations once per
+// k-block.  One (tile, K-slice) unit per CTA, a deep TMA ring (the unit is a chain of k-blocks), one producer warp.
 //   split-K mode : slice z writes raw fp32 partial products to partials[(z * slice_rows + row) * n + feature]
 //                  (same contract as sb_gemm_splitk / sb_gemm_skinny; reduced by sb_splitk_reduce_ln or the attention kernels)
 //   direct mode  : out[row * out_ld + feature] = act(acc + bias) in fp16, act in {none, relu}
@@ -23,7 +21,7 @@ namespace {
 constexpr int DG_BK = 64;
 constexpr int DG_TM = 128;
 constexpr int DG_W_BYTES = DG_TM * DG_BK * 2;
-constexpr int DG_THREADS = 192;  // warps 0-3 epilogue, 4 MMA issuer + TMEM allocator, 5 TMA producer
+constexpr int DG_THREADS = 288;  // warps 0-7 two consumer warpgroups (MMA + epilogue), warp 8 TMA producer
 constexpr int DG_MAX_STAGES = 8;
 
 struct DgArgs {
@@ -34,22 +32,22 @@ struct DgArgs {
   long long slice_rows;
   elem_t* out;
   long long out_ld;
-  const char* prefetch;  // the next kernel's weights: pulled into L2 by an idle epilogue warp
+  const char* prefetch;  // the next kernel's weights: pulled into L2 by the producer warp once its loads are issued
   long long prefetch_bytes;
 };
 
-template <int TCOLS>
+// NT: wgmma N (>= npad).  The activation slot of a stage holds NT rows; TMA fills the first npad (zero past `rows`), the
+// MMA columns beyond them are never stored.
+template <int NT>
 __global__ void __launch_bounds__(DG_THREADS, 1)
 decode_gemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const DgArgs g) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int x_bytes = g.npad * DG_BK * 2, stage_bytes = DG_W_BYTES + x_bytes;
+  constexpr int stage_bytes = DG_W_BYTES + NT * DG_BK * 2;
   uint8_t* misc = smem + (size_t)g.stages * stage_bytes;
   uint64_t* full = (uint64_t*)misc;
   uint64_t* empty = full + DG_MAX_STAGES;
-  uint64_t* tfull = empty + DG_MAX_STAGES;
-  uint32_t* tmem_ptr_smem = (uint32_t*)(tfull + 1);
 
   const int u = blockIdx.x;
   const int tile = u / g.splits, split = u - tile * g.splits;
@@ -58,29 +56,22 @@ decode_gemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmW)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmX)) : "memory");
-    for (int s = 0; s < g.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(tfull, 1);
+    for (int s = 0; s < g.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 4) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "n"(TCOLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == 5) {
+  if (warp == 8) {
     // ---- TMA producer: weights first (they do not depend on the upstream kernel: under PDL they stream while it still runs)
     int s = 0;
     uint32_t ph = 0;
     bool waited = false;
+    const uint32_t tx = (uint32_t)(DG_W_BYTES + g.npad * DG_BK * 2);
     for (int kb = kb0; kb < kb1; ++kb) {
       mbar_wait(&empty[s], ph ^ 1);
       uint8_t* st = smem + (size_t)s * stage_bytes;
       if (elect_one()) {
-        mbar_expect_tx(&full[s], (uint32_t)stage_bytes);
+        mbar_expect_tx(&full[s], tx);
         tma_load_2d(st, &tmW, &full[s], kb * DG_BK, tile * DG_TM);
         if (!waited) pdl_wait();
         tma_load_2d(st + DG_W_BYTES, &tmX, &full[s], kb * DG_BK, 0);
@@ -89,30 +80,7 @@ decode_gemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
       __syncwarp();
       if (++s == g.stages) { s = 0; ph ^= 1; }
     }
-  } else if (warp == 4) {
-    // ---- MMA issuer: D[feature lane][row column] += W[128 x 64] . X[npad x 64]^T
-    const uint32_t idesc = (1u << 4) | ((uint32_t)(g.npad >> 3) << 17) | ((uint32_t)(DG_TM >> 4) << 24);
-    int s = 0;
-    uint32_t ph = 0;
-    for (int kb = kb0; kb < kb1; ++kb) {
-      mbar_wait(&full[s], ph);
-      tc_fence_after();
-      const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
-      const uint64_t da = make_smem_desc(sa), db = make_smem_desc(sa + DG_W_BYTES);
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < DG_BK / 16; ++k)
-          tc_mma_f16(tmem_base, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-        tc_commit(&empty[s]);
-        if (kb == kb1 - 1) tc_commit(tfull);
-      }
-      __syncwarp();
-      if (++s == g.stages) { s = 0; ph ^= 1; }
-    }
-  } else {
-    // ---- epilogue (warps 0-3): TMEM lane = output feature, column = row
-    pdl_sync();
-    if (warp == 0 && g.prefetch_bytes > 0) {
+    if (g.prefetch_bytes > 0) {
       constexpr long long CH = 16384;
       const long long share = ((g.prefetch_bytes + gridDim.x - 1) / gridDim.x + 4095) / 4096 * 4096;
       const long long lo = (long long)blockIdx.x * share, hi = min(lo + share, g.prefetch_bytes);
@@ -121,47 +89,55 @@ decode_gemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
           asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(g.prefetch + o), "r"((uint32_t)min(CH, hi - o)) : "memory");
       __syncwarp();
     }
-    if (kb0 < kb1) {
-      mbar_wait(tfull, 0);
-      tc_fence_after();
-    }
-    const int f = tile * DG_TM + warp * 32 + lane;
-    const bool f_ok = f < g.n_out;
-    const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16);
-    const float bias = (g.partials == nullptr && g.bias != nullptr && f_ok) ? g.bias[f] : 0.f;
-#pragma unroll 1
-    for (int c0 = 0; c0 < g.rows; c0 += 32) {  // warp-uniform
-      uint32_t r[32];
-      if (kb0 < kb1) {
-        tmem_ld32(taddr + (uint32_t)c0, r);
-      } else {
+    return;
+  }
+  // ---- consumers: D[feature][row] += W[64 features of warpgroup wg][64] . X[NT rows][64]^T
+  const int wg = warp >> 2;
+  float acc[NT / 2];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) r[j] = 0u;
-      }
-      if (!f_ok) continue;
-      if (g.partials != nullptr) {
-        float* o = g.partials + ((long long)split * g.slice_rows + c0) * g.n_out + f;
+  for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
+  int s = 0, prev = 0;
+  uint32_t ph = 0;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(&full[s], ph);
+    const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
+    const uint64_t da = make_smem_desc(sa + wg * 64 * 128), db = make_smem_desc(sa + DG_W_BYTES);
+    wg_fence();
 #pragma unroll
-        for (int j = 0; j < 32; ++j)
-          if (c0 + j < g.rows) o[(long long)j * g.n_out] = __uint_as_float(r[j]);
-      } else {
-        elem_t* o = g.out + (long long)c0 * g.out_ld + f;
+    for (int k = 0; k < DG_BK / 16; ++k) Wgmma<NT>::mma(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2));
+    wg_commit();
+    wg_wait<1>();
+    wg_fence_regs(acc);
+    if (kb > kb0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+    prev = s;
+    if (++s == g.stages) { s = 0; ph ^= 1; }
+  }
+  wg_wait<0>();
+  wg_fence_regs(acc);
+  pdl_sync();
+  // ---- epilogue from the accumulator fragment: register j*4 + 2h + e = (feature fb + 8h, row j*8 + 2*(lane%4) + e)
+  const int fb = tile * DG_TM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          if (c0 + j < g.rows) {
-            float v = __uint_as_float(r[j]) + bias;
-            if (g.relu) v = fmaxf(v, 0.f);
-            o[(long long)j * g.out_ld] = __float2half_rn(v);
-          }
+  for (int j = 0; j < NT / 8; ++j) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int f = fb + 8 * h;
+      if (f >= g.n_out) continue;
+      const float bias = (g.partials == nullptr && g.bias != nullptr) ? g.bias[f] : 0.f;
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int r = j * 8 + (lane & 3) * 2 + e;
+        if (r >= g.rows) continue;
+        const float a = acc[j * 4 + 2 * h + e];
+        if (g.partials != nullptr) {
+          g.partials[((long long)split * g.slice_rows + r) * g.n_out + f] = a;
+        } else {
+          float v = a + bias;
+          if (g.relu) v = fmaxf(v, 0.f);
+          g.out[(long long)r * g.out_ld + f] = __float2half_rn(v);
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TCOLS) : "memory");
   }
 }
 
@@ -195,14 +171,14 @@ bool dg_supported(const sb_gemm_t* g, int splits) {
          g->res1 == nullptr && g->res2 == nullptr && g->out2 == nullptr && g->seq_rows == 0;
 }
 
-template <int TCOLS>
+template <int NT>
 int dg_launch(const CUtensorMap& tmW, const CUtensorMap& tmX, const DgArgs& a, int grid, size_t smem, cudaStream_t st) {
   static size_t configured = 0;
   if (smem > configured) {
-    SB_CUDA_OK(cudaFuncSetAttribute(decode_gemm_kernel<TCOLS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    SB_CUDA_OK(cudaFuncSetAttribute(decode_gemm_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = smem;
   }
-  SB_CUDA_OK(launch_k(decode_gemm_kernel<TCOLS>, dim3(grid), dim3(DG_THREADS), smem, st, tmW, tmX, a));
+  SB_CUDA_OK(launch_k(decode_gemm_kernel<NT>, dim3(grid), dim3(DG_THREADS), smem, st, tmW, tmX, a));
   count_launch();
   return SB_OK;
 }
@@ -232,7 +208,8 @@ extern "C" int sb_gemm_decode(const sb_gemm_t* g, int32_t splits, float* partial
   a.out_ld = g->out_ld;
   a.prefetch = (const char*)g->prefetch;
   a.prefetch_bytes = g->prefetch ? g->prefetch_bytes / 4096 * 4096 : 0;
-  const int stage_bytes = DG_W_BYTES + a.npad * DG_BK * 2;
+  const int nt = a.npad <= 32 ? 32 : a.npad <= 64 ? 64 : a.npad <= 128 ? 128 : 256;
+  const int stage_bytes = DG_W_BYTES + nt * DG_BK * 2;
   int dev = 0, smem_optin = 0;
   SB_CUDA_OK(cudaGetDevice(&dev));
   SB_CUDA_OK(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
@@ -251,8 +228,8 @@ extern "C" int sb_gemm_decode(const sb_gemm_t* g, int32_t splits, float* partial
   const int tiles = (g->n + DG_TM - 1) / DG_TM;
   const int grid = tiles * splits;
   cudaStream_t st = (cudaStream_t)stream;
-  if (a.npad <= 32) return dg_launch<32>(tmW, tmX, a, grid, smem, st);
-  if (a.npad <= 64) return dg_launch<64>(tmW, tmX, a, grid, smem, st);
-  if (a.npad <= 128) return dg_launch<128>(tmW, tmX, a, grid, smem, st);
+  if (nt == 32) return dg_launch<32>(tmW, tmX, a, grid, smem, st);
+  if (nt == 64) return dg_launch<64>(tmW, tmX, a, grid, smem, st);
+  if (nt == 128) return dg_launch<128>(tmW, tmX, a, grid, smem, st);
   return dg_launch<256>(tmW, tmX, a, grid, smem, st);
 }

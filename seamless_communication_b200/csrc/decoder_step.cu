@@ -10,8 +10,8 @@
 //     phase in global memory: arrive = fence + atomicAdd, wait = one polling lane per CTA).  Two groups per SM hide each
 //     other's barrier / L2 round trips; the second group's weight tiles hit L2.
 //   * GEMM phases (qkv, attention out, cross q, cross out, FFN inner, FFN out) run "transposed": a 128-feature weight
-//     tile is the tcgen05 A operand, the group's rows are the B operand (N = rows padded to 16), accumulators in
-//     TMEM, both operands staged by TMA (128B swizzle) through one smem ring.  The producer warp runs ahead of the
+//     tile is the wgmma A operand (two m64 halves), the group's rows are the B operand (N = rows padded to 16),
+//     accumulators in the registers of warpgroup 0, both operands staged by TMA (128B swizzle) through one smem ring.  The producer warp runs ahead of the
 //     barriers: the weight tile of a stage is requested as soon as the stage is free, the activation tile only once
 //     the previous phase has completed, so weights stream from HBM while the group waits.
 //     Narrow products split K across CTAs (fp32 partials, reduced in fixed order by the consuming phase).
@@ -37,12 +37,13 @@ constexpr int DS_BK = 64;
 constexpr int DS_TM = 128;
 constexpr int DS_W_BYTES = DS_TM * DS_BK * 2;  // 16 KB weight tile per k-block
 constexpr int DS_WORKERS = 8;
-constexpr int DS_THREADS = 256;                // 8 warps, all SIMT workers; 0-3 also epilogue, 4 MMA issuer, 5 TMA producer
+constexpr int DS_THREADS = 256;                // 8 warps, all SIMT workers; 0-3 also MMA + epilogue, 5 TMA producer
 constexpr int DS_PPL = 11;                     // phases per layer
 constexpr int DS_HD = 64;
 constexpr int DS_MAX_STAGES = 8;
 constexpr int DS_MAX_LAYERS = 32;
-constexpr int DS_MISC_BYTES = 4096;            // barriers, tmem pointer, LN scratch, attention staging (8 x 384 B)
+constexpr int DS_MISC_BYTES = 4096;            // barriers, LN scratch, attention staging (8 x 384 B)
+constexpr int DS_MAX_NPAD = 128;               // rows per group: the wgmma N of the GEMM phases (npad accumulators per thread)
 
 enum { G_QKV = 0, G_OUT = 1, G_CQ = 2, G_CO = 3, G_W1 = 4, G_W2 = 5 };
 // phase offsets inside a layer: GEMM phases are 0,2,4,6,8,9; attention 1,5; reduce + LayerNorm 3,7,10
@@ -100,14 +101,12 @@ __device__ __noinline__ void ds_poll(const unsigned* p, unsigned target) {
   unsigned polls = 0;
   while (ld_relaxed_u32(p) < target) {
     __nanosleep(20);
-    if ((++polls & 4095u) == 0) {  // %globaltimer costs ~1 us per read on B200: the watchdog looks at it every 4096 polls
+    if ((++polls & 4095u) == 0) {  // %globaltimer is slow to read: the watchdog looks at it every 4096 polls
       const unsigned long long now = gtime_ns();
       if (t0 == 0) t0 = now;
-      if (now - t0 > 4000000000ull) {
-        printf("sb_decoder_step: phase barrier timed out (block %d warp %d, have %u want %u)\n", blockIdx.x, threadIdx.x >> 5,
-               ld_relaxed_u32(p), target);
-        __trap();
-      }
+      // a phase barrier that has not completed in 4 s traps (no printf: a call anywhere in the kernel makes ptxas
+      // serialise the wgmma pipeline of the GEMM phases)
+      if (now - t0 > 4000000000ull) asm volatile("trap;");
     }
   }
 }
@@ -172,7 +171,7 @@ __device__ __noinline__ UnitRange unit_range(int u, int splits, int kb_total) {
 }
 
 // Single-query attention of one warp, keys staged in SHARED memory.  A decoder step is a chain of dependent round trips
-// (~1.3 k cycles each under load): reading K/V in register-sized slices put 7+ of them into every attention item.  Here
+// (each a full memory latency under load): reading K/V in register-sized slices put 7+ of them into every attention item.  Here
 // the keys of a pass arrive with one batch of asynchronous copies (cp.async: no registers held) and the arithmetic runs
 // from shared memory: scores -> probabilities (kept in shared memory) -> values, i.e. one round trip for K and one for V.
 // Lane = (key group kg = lane/8, dim chunk dc = lane%8): 4 keys x 128 B per instruction, conflict-free.
@@ -278,12 +277,13 @@ __device__ __forceinline__ void gather_head(const float* __restrict__ part, int 
 }
 
 // ------------------------------------------------------------------------------------------------ the kernel
-// Warp roles: every warp is a SIMT worker; in GEMM phases warps 0-3 run the epilogue (TMEM lane quarter = warp id),
-// warp 4 issues the MMAs, warp 5 is the TMA producer (it requests the next GEMM phase's weight tiles at the tail of
-// the SIMT phase before it, i.e. before that phase's barrier).  8 warps x <= 128 registers keep two CTAs on an SM
-// (registers are per SM sub-partition: 2 CTAs x 2 warps x 128 x 32 = 16 K).
-// TCOLS (TMEM columns, power of two >= 2 * npad) is a compile-time constant.
-template <int TCOLS>
+// Warp roles: every warp is a SIMT worker; in GEMM phases warps 0-3 (warpgroup 0) issue the MMAs and run the epilogue
+// from their accumulator registers, warp 5 is the TMA producer (it requests the next GEMM phase's weight tiles at the
+// tail of the SIMT phase before it, i.e. before that phase's barrier).  8 warps x <= 128 registers keep two CTAs on an
+// SM.  NP (= npad, the wgmma N) is a compile-time constant.  The NP accumulators per warpgroup-0 thread do not fit that
+// budget beside the rest of the kernel for NP >= 64: the sm_90a build spills (stores / loads per thread, bytes): NP 64:
+// 80 / 32, NP 80: 488 / 620, NP 96: 1416 / 1960, NP 128: 2376 / 2720.  The kernel is opt-in (SB_DECODER_FUSED).
+template <int NP>
 __global__ void __launch_bounds__(DS_THREADS, 2) decoder_step_kernel(const __grid_constant__ DsParams P) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -296,44 +296,31 @@ __global__ void __launch_bounds__(DS_THREADS, 2) decoder_step_kernel(const __gri
   const int vc = (blockIdx.x - grp * NC + NC - (grp * NC) / P.G) % NC;
   const int row0 = grp * P.rg;
   const int rg = min(P.rg, P.R - row0);
-  const int npad = P.npad, stages = P.stages;
-  const int x_bytes = npad * DS_BK * 2, stage_bytes = DS_W_BYTES + x_bytes;
+  const int stages = P.stages;
+  constexpr int stage_bytes = DS_W_BYTES + NP * DS_BK * 2;
   unsigned* cnt = P.counters + (size_t)grp * P.n_phases;
   unsigned long long* tl = (P.timeline != nullptr && vc == 0) ? P.timeline + (size_t)grp * P.n_phases * 8 : nullptr;
   uint8_t* ring = smem;
   uint8_t* misc = smem + (size_t)stages * stage_bytes;
   uint64_t* full = (uint64_t*)misc;
   uint64_t* empty = full + DS_MAX_STAGES;
-  uint64_t* tfull = empty + DS_MAX_STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_ptr_smem = (uint32_t*)(tempty + 2);
   float* s_red = (float*)(misc + 512);                           // [2][2][8] floats
   elem_t* stage_s = (elem_t*)(misc + 1024) + warp * 3 * DS_HD;   // per-warp [3][64] halves: q | k | v of the new token
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], 4); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 4) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "n"(TCOLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   const int dim = P.dim, H = P.heads;
   const int step = *P.step_ptr;
   // per-role running state
-  uint32_t unit_ctr = 0;                   // accumulator parity: epilogue warps and the MMA warp count units identically
-  int mma_stage = 0;                       // warp 4: ring stage / parity of the next slot
+  int mma_stage = 0;                       // warpgroup 0: ring stage / parity of the next slot
   uint32_t mma_parity = 0;
   int w_stage = 0, x_stage = 0;            // warp 5: ring cursors of the weight / activation requests
   uint32_t w_parity = 0;
   int pre_phase = -1, pre_n = 0;           // warp 5: phase whose first pre_n weight tiles are already requested
-  const uint32_t idesc = (1u << 4) | ((uint32_t)(npad >> 3) << 17) | ((uint32_t)(DS_TM >> 4) << 24);  // D=f32, A=B=f16, K-major, N>>3, M>>4
 
   // weight tile (k-block kb, rows w_row..) -> next ring stage (waits for the stage to be free)
   auto issue_w = [&](const CUtensorMap* tm, int kb, int w_row) {
@@ -373,8 +360,6 @@ __global__ void __launch_bounds__(DS_THREADS, 2) decoder_step_kernel(const __gri
       for (int u = vc; u < units; u += NC) {
         const UnitRange ur = unit_range(u, g.splits, g.kb_total);
         if (ur.kb0 >= ur.kb1) continue;
-        const uint32_t acc = unit_ctr & 1, acc_ph = (unit_ctr >> 1) & 1;
-        ++unit_ctr;
         if (warp == 5) {
           // ---- TMA producer
 #pragma unroll 1
@@ -392,59 +377,63 @@ __global__ void __launch_bounds__(DS_THREADS, 2) decoder_step_kernel(const __gri
             if (++x_stage == stages) x_stage = 0;
           }
           if (lane == 0) DS_TL(p, 3);
-        } else if (warp == 4) {
-          // ---- MMA issuer
-          mbar_wait(&tempty[acc], acc_ph ^ 1);
-          tc_fence_after();
-          const uint32_t d_addr = tmem_base + acc * (uint32_t)npad;
+        } else if (warp < 4) {
+          // ---- MMA: D[feature][row] += W[128 x 64] . X[NP x 64]^T, features 0-63 in acc[0], 64-127 in acc[1]
+          float acc[2][NP / 2];
+#pragma unroll
+          for (int i = 0; i < NP / 2; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+          int prev = 0;
 #pragma unroll 1
           for (int kb = ur.kb0; kb < ur.kb1; ++kb) {
             const int s = mma_stage;
             mbar_wait(&full[s], mma_parity);
             if (++mma_stage == stages) { mma_stage = 0; mma_parity ^= 1; }
-            tc_fence_after();
-            if (kb == ur.kb0 && lane == 0) DS_TL(p, 6);
+            if (kb == ur.kb0 && threadIdx.x == 0) DS_TL(p, 6);
             const uint32_t sa = smem_u32(ring + (size_t)s * stage_bytes);
             const uint64_t da = make_smem_desc(sa), db = make_smem_desc(sa + DS_W_BYTES);
-            if (elect_one()) {
+            wg_fence();
 #pragma unroll
-              for (int kk = 0; kk < DS_BK / 16; ++kk)
-                tc_mma_f16(d_addr, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), idesc, (kb > ur.kb0 || kk > 0) ? 1u : 0u);
-              tc_commit(&empty[s]);
-              if (kb == ur.kb1 - 1) tc_commit(&tfull[acc]);
+            for (int kk = 0; kk < DS_BK / 16; ++kk) {
+              Wgmma<NP>::mma(acc[0], da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2));
+              Wgmma<NP>::mma(acc[1], da + (uint64_t)(64 * 128 / 16 + kk * 2), db + (uint64_t)(kk * 2));
             }
-            __syncwarp();
+            wg_commit();
+            wg_wait<1>();
+            wg_fence_regs(acc[0]);
+            wg_fence_regs(acc[1]);
+            if (kb > ur.kb0 && threadIdx.x == 0) mbar_arrive(&empty[prev]);
+            prev = s;
           }
-        } else if (warp < 4) {
-          // ---- epilogue: TMEM lane = output feature, column = row of the group
-          mbar_wait(&tfull[acc], acc_ph);
-          tc_fence_after();
+          wg_wait<0>();
+          wg_fence_regs(acc[0]);
+          wg_fence_regs(acc[1]);
+          if (threadIdx.x == 0) mbar_arrive(&empty[prev]);
           if (threadIdx.x == 0) DS_TL(p, 2);
-          const int f = ur.tile * DS_TM + warp * 32 + lane;
-          const bool f_ok = f < g.n_out;
-          const float bias = (g.relu_f16 && f_ok) ? L.bias[G_W1][f] : 0.f;
-          const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + acc * (uint32_t)npad;
-          // byte address of (first row of the group, feature f) in the output; rows are n_out elements apart
+          // ---- epilogue: register j*4 + 2h + e of acc[mt] = (feature fb + 64 mt + 8h, row j*8 + 2*(lane%4) + e of the group)
+          const int fb = ur.tile * DS_TM + warp * 16 + (lane >> 2);
           const int esz = g.relu_f16 ? 2 : 4;
-          char* o = reinterpret_cast<char*>(g.out) + (((size_t)(g.relu_f16 ? 0 : ur.split) * P.R + row0) * g.n_out + f) * esz;
-          const size_t rstride = (size_t)g.n_out * esz;
-#pragma unroll 1
-          for (int c0 = 0; c0 < rg; c0 += 16, o += 16 * rstride) {
-            uint32_t r[16];
-            tmem_ld16(taddr + (uint32_t)c0, r);
-            const int nj = f_ok ? rg - c0 : 0;
+          char* o = reinterpret_cast<char*>(g.out) + ((size_t)(g.relu_f16 ? 0 : ur.split) * P.R + row0) * g.n_out * esz;
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              if (j < nj) {
-                const float v = __uint_as_float(r[j]);
-                if (g.relu_f16) *reinterpret_cast<elem_t*>(o + j * rstride) = __float2half_rn(fmaxf(v + bias, 0.f));
-                else *reinterpret_cast<float*>(o + j * rstride) = v;
+          for (int mt = 0; mt < 2; ++mt) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int f = fb + 64 * mt + 8 * h;
+              if (f >= g.n_out) continue;
+              const float bias = g.relu_f16 ? L.bias[G_W1][f] : 0.f;
+#pragma unroll
+              for (int j = 0; j < NP / 8; ++j) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const int r = j * 8 + (lane & 3) * 2 + e;
+                  if (r >= rg) continue;
+                  const float v = acc[mt][j * 4 + 2 * h + e];
+                  char* d = o + ((size_t)r * g.n_out + f) * esz;
+                  if (g.relu_f16) *reinterpret_cast<elem_t*>(d) = __float2half_rn(fmaxf(v + bias, 0.f));
+                  else *reinterpret_cast<float*>(d) = v;
+                }
               }
             }
           }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty[acc]);
         }
       }
       if (warp < 4) {
@@ -662,12 +651,6 @@ __global__ void __launch_bounds__(DS_THREADS, 2) decoder_step_kernel(const __gri
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TCOLS) : "memory");
-  }
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -698,12 +681,16 @@ int encode_map(CUtensorMap* tm, const void* base, uint64_t inner, uint64_t rows,
 
 typedef void (*DsKernel)(DsParams);
 DsKernel pick_kernel(int npad) {
-  const int need = 2 * npad;
-  if (need <= 32) return decoder_step_kernel<32>;
-  if (need <= 64) return decoder_step_kernel<64>;
-  if (need <= 128) return decoder_step_kernel<128>;
-  if (need <= 256) return decoder_step_kernel<256>;
-  return decoder_step_kernel<512>;
+  switch (npad) {
+    case 16: return decoder_step_kernel<16>;
+    case 32: return decoder_step_kernel<32>;
+    case 48: return decoder_step_kernel<48>;
+    case 64: return decoder_step_kernel<64>;
+    case 80: return decoder_step_kernel<80>;
+    case 96: return decoder_step_kernel<96>;
+    case 112: return decoder_step_kernel<112>;
+    default: return decoder_step_kernel<128>;
+  }
 }
 
 int env_int(const char* name, int dflt) {
@@ -761,9 +748,9 @@ extern "C" int sb_decoder_plan_query(int32_t layers, int32_t dim, int32_t ffn_di
   if (G > 2) G = 2;
   if (G > rows) G = 1;
   int rg = (rows + G - 1) / G;
-  if (rg > 256) { G = 2; rg = (rows + 1) / 2; }
+  if (rg > DS_MAX_NPAD) { G = 2; rg = (rows + 1) / 2; }
   if (beam > 1) rg = (rg + beam - 1) / beam * beam;  // groups hold whole sentences (cross-attention shares K/V across the beams)
-  SB_REQUIRE(rg <= 256, SB_ENOSUP, "sb_decoder_plan_query: %d rows exceed 2 groups x 256", rows);
+  SB_REQUIRE(rg <= DS_MAX_NPAD, SB_ENOSUP, "sb_decoder_plan_query: %d rows exceed 2 groups x %d", rows, DS_MAX_NPAD);
   const int npad = (rg + 15) / 16 * 16;
   const int stage_bytes = DS_W_BYTES + npad * DS_BK * 2;
   // every resident CTA also pays 1 KB of system shared memory
@@ -879,10 +866,7 @@ extern "C" int sb_decoder_plan_init(const sb_decoder_plan_desc_t* d, sb_decoder_
     SB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
     SB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   }
-  // Co-residency of all groups x NC CTAs is required (phase barriers spin).  cudaOccupancyMaxActiveBlocksPerMultiprocessor
-  // cannot be used: for any kernel containing tcgen05.alloc it reports 1 block (0 with dynamic shared memory) on CUDA 12.9
-  // (tools/probes/occ_probe.cu), while the hardware limits (ncu launch__occupancy_limit_*) are registers / shared memory
-  // / TMEM columns only.  Check those here.
+  // Co-residency of all groups x NC CTAs is required (phase barriers spin): check registers and shared memory per SM.
   {
     cudaFuncAttributes fa;
     SB_CUDA_OK(cudaFuncGetAttributes(&fa, kern));
@@ -891,12 +875,9 @@ extern "C" int sb_decoder_plan_init(const sb_decoder_plan_desc_t* d, sb_decoder_
     SB_CUDA_OK(cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev));
     SB_CUDA_OK(cudaDeviceGetAttribute(&regs_sm, cudaDevAttrMaxRegistersPerMultiprocessor, dev));
     const int regs_cta = ((fa.numRegs + 7) / 8 * 8) * DS_THREADS;
-    int tcols = 32;
-    while (tcols < 2 * info.npad) tcols <<= 1;
-    SB_REQUIRE(info.groups * regs_cta <= regs_sm && info.groups * (info.smem_bytes + 1024 + (int)fa.sharedSizeBytes) <= smem_sm &&
-                   info.groups * tcols <= 512,
-               SB_ENOSUP, "sb_decoder_plan_init: %d CTAs per SM do not fit (regs %d x %d threads, smem %d B, %d TMEM columns)",
-               info.groups, fa.numRegs, DS_THREADS, info.smem_bytes, tcols);
+    SB_REQUIRE(info.groups * regs_cta <= regs_sm && info.groups * (info.smem_bytes + 1024 + (int)fa.sharedSizeBytes) <= smem_sm,
+               SB_ENOSUP, "sb_decoder_plan_init: %d CTAs per SM do not fit (regs %d x %d threads, smem %d B)",
+               info.groups, fa.numRegs, DS_THREADS, info.smem_bytes);
   }
   launch->npad = info.npad;
   launch->counters = d->counters;
@@ -904,9 +885,8 @@ extern "C" int sb_decoder_plan_init(const sb_decoder_plan_desc_t* d, sb_decoder_
   launch->grid = info.groups * info.ctas_per_group;
   launch->block = DS_THREADS;
   launch->smem_bytes = info.smem_bytes;
-  // the cooperative-launch size check shares the occupancy calculator's blind spot: with 2 CTAs per SM it would be
-  // refused, so two-group plans use a plain launch (the resource check above + an otherwise idle stream order guarantee
-  // residency; every spin in the kernel is bounded)
+  // two-group plans use a plain launch (the resource check above + an otherwise idle stream order guarantee residency;
+  // every spin in the kernel is bounded)
   launch->cooperative = env_int("SB_DS_COOPERATIVE", info.groups == 1 ? 1 : 0);
   return SB_OK;
 }

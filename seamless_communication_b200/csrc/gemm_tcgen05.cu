@@ -1,16 +1,13 @@
-// sb_gemm: fused Linear / Conv1d-as-GEMM for sm_100a.
+// sb_gemm: fused Linear / Conv1d-as-GEMM for sm_90a.
 //
-//   TMA (cp.async.bulk.tensor, 128B swizzle) -> 3/4-stage smem ring -> tcgen05.mma (kind::f16, fp32 accumulate in
-//   TMEM, issued by one thread) -> tcgen05.ld epilogue (bias, activation / GLU, residuals, sequence mask, fp16|fp32
-//   store, optional leaky-relu'd second output).
+//   TMA (cp.async.bulk.tensor, 128B swizzle) -> 3/4-stage smem ring -> wgmma (m64nBNk16, fp16 in, fp32 accumulate in
+//   registers of two consumer warpgroups, 64 tile rows each) -> fp32 tile staged in the drained ring -> epilogue (bias,
+//   activation / GLU, residuals, sequence mask, fp16|fp32 store, optional leaky-relu'd second output).
 //
-// Warp roles: warps 0-3 epilogue (TMEM lane quarter = warp id), warp 4 MMA issuer + TMEM allocator, warps 5.. TMA
-// producers - ONE PRODUCER PER PIPELINE STAGE.  Measured on B200 (tools/tma_probe.py, profiles/r01_tma_probe.txt):
-// a single thread sustains only one wait-empty / expect-tx / cp.async.bulk.tensor round per ~650 cycles no matter
-// how many stages are in flight, so a lone producer caps a CTA at ~25 B/clk; one producer per stage multiplies that.
-// One 128 x BN output tile per CTA; 2 CTAs co-reside per SM (<= 96 KB smem, <= 128 TMEM columns each) so one CTA's
-// epilogue overlaps the other's main loop.  The epilogue stages the tile in shared memory (128B-swizzled, conflict
-// free) and writes it with TMA bulk stores (full 128 B rows; tile tails are clipped by the tensor map).
+// Warp roles: warps 0-7 consumers (warpgroup = 64 tile rows; warps 0-3 then run the epilogue, one tile row per
+// thread), warp 8 TMA producer.  One 128 x BN output tile per CTA; up to BN = 128 two CTAs co-reside per SM so one
+// CTA's epilogue overlaps the other's main loop.  The epilogue stages the output tile in shared memory (128B-swizzled,
+// conflict free) and writes it with TMA bulk stores (full 128 B rows; tile tails are clipped by the tensor map).
 //
 // Conv taps are realised purely through the TMA row coordinate: tap j of output row m reads A row
 // a_row0 + m + j*dil, the weight K index is j*c_in + c.  Rows outside [0, a_rows) and channels >= c_in are
@@ -56,32 +53,26 @@ struct GemmArgs {
   long long prefetch_bytes;
 };
 
-template <int BN, bool DEEP = false>
+template <int BN>
 struct TileCfg {
-  // DEEP: one CTA per SM with as many stages as fit - for skinny problems (few CTAs) whose K loop is a chain of
-  // ~1.4 us load round trips (tools/gemm_timeline.py); the default keeps 2 CTAs/SM so epilogues overlap main loops
-  // BN = 256: two stages of 48 KB keep 2 CTAs/SM (TMEM 2 x 256 columns) while every A tile feeds twice the columns:
-  // 85 instead of 64 FLOP per byte moved L2 -> SM, the bound of the 128-wide tiles (profiles/r01_notes.md)
-  static constexpr int STAGES = DEEP ? (BN >= 128 ? 6 : 8) : (BN >= 256 ? 2 : (BN >= 128) ? 3 : 4);
+  // BN <= 128: two CTAs per SM (<= 113 KB of shared memory each) so that one CTA's epilogue overlaps the other's main
+  // loop.  BN = 256: every A tile feeds twice the columns (85 instead of 64 FLOP per byte moved L2 -> SM); its 128 x 256
+  // fp32 accumulator needs 128 registers per consumer thread and 128 KB of staging, so it runs one CTA per SM.
+  static constexpr int STAGES = BN >= 128 ? 3 : 4;
+  static constexpr int MIN_CTAS = BN >= 256 ? 1 : 2;
   static constexpr int B_TILE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_TILE_BYTES + B_TILE_BYTES;
-  // Accumulating tcgen05.mma instructions that target the same TMEM tile issue ~180 cycles apart (measured:
-  // 0.38 us per 64-deep k-block = 4 dependent MMAs, independent of N, tools/gemm_timeline.py), while a 128xBNx16 MMA
-  // keeps the tensor pipe busy for only BN/2 cycles.  The K loop therefore round-robins NACC independent accumulators
-  // (summed in the epilogue) so that several MMA chains are in flight.
-  // (Measured in round 1: with MMA issue already under elect.sync the extra accumulators bought nothing and cost
-  // epilogue TMEM reads, so NACC is 1; the mechanism stays for the 256-wide 2-CTA tiles planned next.)
-  static constexpr int NACC = 1;
-  static constexpr int TMEM_COLS = NACC * BN < 32 ? 32 : NACC * BN;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + BN * 4;
-  static constexpr int THREADS = 32 * (5 + STAGES);
-  // epilogue staging reuses the (drained) pipeline stages: out groups first, out2 groups after them
+  static constexpr int THREADS = 32 * 9;  // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+  // After the main loop the drained ring holds the fp32 accumulator tile: 16 KB chunks of [128 rows][32 columns], 16-byte
+  // units XOR (row & 7).  The epilogue stages its outputs in place (out groups of chunk c land in chunks <= c of the same
+  // row, already read by the thread that owns the row); out2 groups follow the accumulator chunks.
   // fp32 worst case: 32 columns per 16 KB group; the 256-wide tile stages fp16 outputs only (no fp32 / second output: the
   // host never selects it for those)
   static constexpr int OUT_GROUPS_MAX = BN >= 256 ? BN * 2 / 128 : BN * 4 / 128;
   static constexpr int OUT2_OFFSET = OUT_GROUPS_MAX * 16384;
+  static_assert(BM * BN * 4 <= STAGES * STAGE_BYTES, "accumulator staging does not fit");
   static_assert(BN >= 256 || OUT2_OFFSET + (BN / 64 > 0 ? BN / 64 : 1) * 16384 <= STAGES * STAGE_BYTES, "staging does not fit");
-  static_assert(OUT_GROUPS_MAX * 16384 <= STAGES * STAGE_BYTES, "staging does not fit");
 };
 
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, const void* smem_src, int c0, int c1) {
@@ -94,23 +85,21 @@ __device__ unsigned long long* g_timeline = nullptr;
 __device__ __forceinline__ unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
 #define TL(i) do { if (g_timeline != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0) g_timeline[i] = gtime(); } while (0)
 
-template <int BN, bool DEEP>
-__global__ void __launch_bounds__(TileCfg<BN, DEEP>::THREADS, DEEP ? 1 : 2)
+template <int BN>
+__global__ void __launch_bounds__(TileCfg<BN>::THREADS, TileCfg<BN>::MIN_CTAS)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmO2, const GemmArgs g) {
-  using Cfg = TileCfg<BN, DEEP>;
+  using Cfg = TileCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = (uint64_t*)(smem + STAGES * Cfg::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_ptr_smem = (uint32_t*)(tmem_full_bar + 1);
   float* bias_s = (float*)(smem + STAGES * Cfg::STAGE_BYTES + 256);
 
   if (threadIdx.x == 0) {
     TL(0);
-    // hide the descriptor fetch of the first TMA behind the barrier / TMEM setup
+    // hide the descriptor fetch of the first TMA behind the barrier setup
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmW)) : "memory");
     if (g.tma_store) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmO)) : "memory");
@@ -127,16 +116,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);  // one arrival per consumer warpgroup
     }
-    mbar_init(tmem_full_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 4) {  // TMEM allocation (whole warp), address lands in smem
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)),
-                 "r"((uint32_t)Cfg::TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   if (warp < 4) {
     for (int i = threadIdx.x; i < BN; i += 128) {
@@ -144,76 +126,33 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       bias_s[i] = (g.bias != nullptr && n < g.n) ? g.bias[n] : 0.f;
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   if (threadIdx.x == 0) TL(1);
 
-  if (warp >= 5) {
-    // ------------------------------------------------------------------ TMA producers: warp 5+s owns stage s
-    {
-      const int s = warp - 5;
+  if (warp == 8) {
+    // ------------------------------------------------------------------ TMA producer
+    int s = 0;
+    uint32_t ph = 0;
+    for (int kr = 0; kr < kblocks; ++kr) {
+      mbar_wait(&empty_bar[s], ph ^ 1);
       uint8_t* sa = smem + s * Cfg::STAGE_BYTES;
-      uint32_t ph = 0;
-      for (int kr = s; kr < kblocks; kr += STAGES, ph ^= 1) {
-        mbar_wait(&empty_bar[s], ph ^ 1);
-        const int kb = kb_begin + kr;
-        const int tap = kb / cblocks, c0 = (kb - tap * cblocks) * BK;
-        if (elect_one()) {
-          mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
-          // weights first: they do not depend on the upstream kernel, so under PDL they stream while it still runs
-          tma_load_2d(sa + A_TILE_BYTES, &tmW, &full_bar[s], tap * g.c_in + c0, n0);
-          if (kr == s) pdl_wait();
-          tma_load_2d(sa, &tmA, &full_bar[s], c0, m0 + g.a_row0 + tap * g.dil);
-        }
-        __syncwarp();
+      const int kb = kb_begin + kr;
+      const int tap = kb / cblocks, c0 = (kb - tap * cblocks) * BK;
+      if (elect_one()) {
+        if (kr == 0) TL(2);
+        mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
+        // weights first: they do not depend on the upstream kernel, so under PDL they stream while it still runs
+        tma_load_2d(sa + A_TILE_BYTES, &tmW, &full_bar[s], tap * g.c_in + c0, n0);
+        if (kr == 0) pdl_wait();
+        tma_load_2d(sa, &tmA, &full_bar[s], c0, m0 + g.a_row0 + tap * g.dil);
       }
+      __syncwarp();
+      if (++s == STAGES) { s = 0; ph ^= 1; }
     }
-  } else if (warp == 4) {
-    // ------------------------------------------------------------------ MMA issuer (whole warp converged, one lane issues)
-    {
-      // instruction descriptor: D=f32, A=B=f16 (0) / bf16 (1), K-major both, N>>3, M>>4
-      const uint32_t idesc = (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-      int s = 0, cb = kb_begin % cblocks;
-      uint32_t ph = 0;
-      uint32_t kstep = 0;  // running k-step index: accumulator kstep % NACC, first touch of each accumulator overwrites
-      for (int kb = 0; kb < kblocks; ++kb) {
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + s * Cfg::STAGE_BYTES);
-        const uint64_t da = make_smem_desc(sa), db = make_smem_desc(sa + A_TILE_BYTES);
-        int ksteps = (g.c_in - cb * BK + 15) >> 4;
-        if (ksteps > BK / 16) ksteps = BK / 16;
-        if (++cb == cblocks) cb = 0;
-        if (elect_one()) {
-          if (kb == 0) TL(2);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            if (k < ksteps) {
-              // advance 16 elements (32 B) along K inside the swizzle atom: +2 in the (addr >> 4) field
-              tc_mma_f16(tmem_base + ((kstep + k) % Cfg::NACC) * BN, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc,
-                         (kstep + k) >= (uint32_t)Cfg::NACC);
-            }
-          }
-          tc_commit(&empty_bar[s]);  // frees the smem stage once these MMAs have read it
-          if (kb == kblocks - 1) {
-            tc_commit(tmem_full_bar);  // accumulators complete
-            TL(3);
-          }
-        }
-        __syncwarp();
-        kstep += ksteps;
-        if (++s == STAGES) { s = 0; ph ^= 1; }
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue (warps 0..3)
-    pdl_sync();  // residual reads / output writes below must not overtake the upstream kernel; dependents may launch now
-    if (warp == 0 && g.prefetch_bytes > 0) {
+    if (g.prefetch_bytes > 0) {
       // latency-bound chains (decoder step): the next GEMM's weights do not depend on this kernel's result, so each CTA
-      // asks L2 for its share now; the next kernel's first TMA loads then hit L2 instead of paying an HBM round trip
-      // (UBLKPF is a uniform-datapath instruction: one elected lane issues, in 16 KB pieces of this CTA's contiguous share)
+      // asks L2 for its share once its own loads are issued; the next kernel's first TMA loads then hit L2 instead of
+      // paying an HBM round trip (one elected lane issues, in 16 KB pieces of this CTA's contiguous share)
       constexpr long long CH = 16384;
       const long long cta = blockIdx.x + (long long)gridDim.x * (blockIdx.y + (long long)gridDim.y * blockIdx.z);
       const long long ncta = (long long)gridDim.x * gridDim.y * gridDim.z;
@@ -225,9 +164,54 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
       __syncwarp();
     }
-    mbar_wait(tmem_full_bar, 0);
+    return;
+  }
+  // -------------------------------------------------------------------- consumers: warpgroup wg owns tile rows [64 wg, 64 wg + 64)
+  {
+    const int wg = warp >> 2;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int s = 0, prev = 0;
+    uint32_t ph = 0;
+    for (int kb = 0; kb < kblocks; ++kb) {
+      mbar_wait(&full_bar[s], ph);
+      const uint32_t sa = smem_u32(smem + s * Cfg::STAGE_BYTES);
+      const uint64_t da = make_smem_desc(sa + wg * (BM / 2) * 128), db = make_smem_desc(sa + A_TILE_BYTES);
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) Wgmma<BN>::mma(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2));
+      wg_commit();
+      // the previous k-block's MMAs have read their stage once at most this block's group is in flight.  (Channels past
+      // c_in are zero-filled by TMA, so a partial last channel block contributes exact zeros.)
+      wg_wait<1>();
+      wg_fence_regs(acc);
+      if (kb > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+      prev = s;
+      if (++s == STAGES) { s = 0; ph ^= 1; }
+    }
+    wg_wait<0>();
+    wg_fence_regs(acc);
+    if (threadIdx.x == 0) TL(3);
+    // every MMA of both warpgroups has read the ring: it now stages the fp32 tile (layout: see TileCfg)
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = r0 + 8 * h, col = j * 8 + (lane & 3) * 2;
+        *reinterpret_cast<float2*>(smem + (col >> 5) * 16384 + r * 128 + ((((col & 31) >> 2) ^ (r & 7)) << 4) + (col & 3) * 4) =
+            make_float2(acc[j * 4 + 2 * h], acc[j * 4 + 2 * h + 1]);
+      }
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+  }
+  if (warp >= 4) return;
+  {
+    // ------------------------------------------------------------------ epilogue (warps 0..3, one tile row per thread)
+    pdl_sync();  // residual reads / output writes below must not overtake the upstream kernel; dependents may launch now
     if (threadIdx.x == 0) TL(4);
-    tc_fence_after();
     const int row = warp * 32 + lane;
     const long long m = (long long)m0 + row;
     const bool row_ok = m < g.m;
@@ -235,13 +219,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const bool valid = row_ok && seq_row_valid(q, g.seq_rows, g.seq_halo, g.seq_len, g.seq_lens);
     const int n_out_total = g.glu ? g.n / 2 : g.n;
     // NOTE: every access to v[] below uses compile-time indices (fully unrolled loops with predicates); a single
-    // runtime-indexed access would push the whole array to local memory (seen in profiles/r01_gemm_v1_*.txt).
-    // accumulators that received at least one MMA: min(NACC, #k-steps of this CTA); the last channel block of a tap
-    // may hold fewer than 4 k-steps when c_in is not a multiple of 64
-    const int tail_steps = (g.c_in - (cblocks - 1) * BK + 15) >> 4;
-    const int n_tail = kb_stop / cblocks - kb_begin / cblocks;
-    const int total_steps = (BK / 16) * (kblocks - n_tail) + tail_steps * n_tail;
-    const int n_acc = total_steps < Cfg::NACC ? total_steps : Cfg::NACC;
+    // runtime-indexed access would push the whole array to local memory.
     const bool has_res = valid && (g.res1 != nullptr || g.res2 != nullptr);
     const float post_scale = has_res ? g.gamma : g.alpha * g.gamma;
     float st_m = -INFINITY, st_s = 0.f;  // running log-sum-exp statistics of this thread's row (tile_stats)
@@ -249,16 +227,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     for (int c0 = 0; c0 < BN; c0 += 32) {
       if (n0 + c0 >= g.n) break;  // warp-uniform
       float v[32];
+      const uint8_t* ap = smem + (c0 >> 5) * 16384 + row * 128;
 #pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = bias_s[c0 + j];
-#pragma unroll
-      for (int a = 0; a < Cfg::NACC; ++a) {
-        if (a < n_acc) {  // warp-uniform
-          uint32_t r[32];
-          tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(a * BN + c0), r);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += __uint_as_float(r[j]);
-        }
+      for (int j = 0; j < 8; ++j) {
+        const float4 a = *reinterpret_cast<const float4*>(ap + ((j ^ (row & 7)) << 4));
+        v[4 * j] = a.x + bias_s[c0 + 4 * j];
+        v[4 * j + 1] = a.y + bias_s[c0 + 4 * j + 1];
+        v[4 * j + 2] = a.z + bias_s[c0 + 4 * j + 2];
+        v[4 * j + 3] = a.w + bias_s[c0 + 4 * j + 3];
       }
       if (!row_ok) continue;
       int nv = 32;         // number of output values in this chunk
@@ -414,7 +390,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (g.tma_store) {
       // make the staged tile visible to the async proxy, then one thread issues the bulk tensor stores
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("bar.sync 1, 128;" ::: "memory");
+      asm volatile("bar.sync 2, 128;" ::: "memory");
       if (threadIdx.x == 0) {
         const int n_tile_out = g.glu ? BN / 2 : BN;
         const int oc0 = g.glu ? (n0 >> 1) : n0;
@@ -431,14 +407,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
   }
   if (threadIdx.x == 0) TL(5);
-  tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x == 0) TL(6);
-  if (warp == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)Cfg::TMEM_COLS)
-                 : "memory");
-  }
 }
 
 // ---------------------------------------------------------------------------------------------- host side
@@ -475,6 +443,19 @@ static int make_tmap(CUtensorMap* tm, const void* base, uint64_t inner, uint64_t
   return SB_OK;
 }
 
+// SMs of the current device (tile-size choice); cached per device
+int sm_count() {
+  static int cached[64] = {0};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+  if (cached[dev] == 0) {
+    int n = 0;
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    cached[dev] = n > 0 ? n : 132;
+  }
+  return cached[dev];
+}
+
 static int validate(const sb_gemm_t* g) {
   SB_REQUIRE(g != nullptr && g->a != nullptr && g->w != nullptr && g->out != nullptr, SB_EINVAL, "sb_gemm: null operand");
   SB_REQUIRE(g->m > 0 && g->n > 0 && g->c_in > 0 && g->taps > 0, SB_EINVAL, "sb_gemm: bad shape m=%d n=%d c_in=%d taps=%d",
@@ -503,12 +484,12 @@ static void fill_args(const sb_gemm_t* g, GemmArgs* a) {
   a->m_fast = 0;
 }
 
-template <int BN, bool DEEP = false>
+template <int BN>
 static int launch(const sb_gemm_t* g, cudaStream_t st, int splits = 1, long long slice_rows = 0) {
-  using Cfg = TileCfg<BN, DEEP>;
+  using Cfg = TileCfg<BN>;
   static bool configured = false;
   if (!configured) {
-    SB_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BN, DEEP>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    SB_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     configured = true;
   }
   CUtensorMap tmA, tmW, tmO, tmO2;
@@ -561,7 +542,7 @@ static int launch(const sb_gemm_t* g, cudaStream_t st, int splits = 1, long long
     args.m_fast = 1;
     grid = dim3(grid.y, grid.x, grid.z);
   }
-  SB_CUDA_OK(launch_k(gemm_tc_kernel<BN, DEEP>, grid, dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, tmA, tmW, tmO, tmO2, args));
+  SB_CUDA_OK(launch_k(gemm_tc_kernel<BN>, grid, dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, tmA, tmW, tmO, tmO2, args));
   count_launch();
   return SB_OK;
 }
@@ -628,6 +609,7 @@ extern "C" int sb_gemm(const sb_gemm_t* g_in, sb_stream_t stream) {
     g = &gc;
   }
   const long long mt = (g->m + sb::BM - 1) / sb::BM;
+  const int sms = sb::sm_count();
   auto tiles = [&](int bn) { return mt * ((g->n + bn - 1) / bn); };
   if (g->tile_stats != nullptr) {
     SB_REQUIRE(!g->glu && g->n >= 128, SB_ENOSUP, "sb_gemm: tile_stats needs n >= 128 and no GLU");
@@ -636,10 +618,10 @@ extern "C" int sb_gemm(const sb_gemm_t* g_in, sb_stream_t stream) {
   // 256-wide tiles for the large products (encoder / T2U / vocoder GEMMs): fp16 single-output epilogues, whole tiles only
   const char* e256 = getenv("SB_GEMM_BN256");  // read per call: tools toggle it inside one process
   const int bn256 = (e256 == nullptr || atoi(e256) != 0) ? 1 : 0;
-  if (bn256 && (g->n % 256) == 0 && !g->out_f32 && g->out2 == nullptr && tiles(256) >= 2 * 148) return sb::launch<256>(g, st);
-  // largest N tile that still gives every SM two CTAs; fall back to smaller tiles for skinny problems
-  if (g->n >= 128 && tiles(128) >= 148) return sb::launch<128>(g, st);
-  if (g->n >= 64 && tiles(64) >= 148) return sb::launch<64>(g, st);
+  if (bn256 && (g->n % 256) == 0 && !g->out_f32 && g->out2 == nullptr && tiles(256) >= 2 * sms) return sb::launch<256>(g, st);
+  // largest N tile that still gives every SM a CTA; fall back to smaller tiles for skinny problems
+  if (g->n >= 128 && tiles(128) >= sms) return sb::launch<128>(g, st);
+  if (g->n >= 64 && tiles(64) >= sms) return sb::launch<64>(g, st);
   if (g->n > 64) return sb::launch<64>(g, st);
   return sb::launch<32>(g, st);
 }

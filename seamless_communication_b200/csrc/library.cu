@@ -10,7 +10,7 @@ static thread_local char g_err[512] = "";
 long long g_launch_count = 0;
 bool pdl_enabled() {
   static int v = -1;
-  // opt-in (SB_PDL=1): measured slower than plain graph edges on B200 in round 1 (profiles/r01_notes.md)
+  // opt-in (SB_PDL=1; not timed on H100)
   if (v < 0) { const char* e = getenv("SB_PDL"); v = (e != nullptr && atoi(e) != 0) ? 1 : 0; }
   return v != 0;
 }
@@ -36,7 +36,7 @@ extern "C" int sb_cast_f32_to_f16(const float* src, void* dst, int64_t n, sb_str
   SB_REQUIRE(src && dst && n >= 0, SB_EINVAL, "sb_cast_f32_to_f16: bad args");
   if (n == 0) return SB_OK;
   long long blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > (long long)sb::sm_count() * 16) blocks = (long long)sb::sm_count() * 16;  // grid-stride loop
   sb::cast_f32_f16_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(src, (sb::elem_t*)dst, n);
   SB_LAUNCH_OK();
   return SB_OK;

@@ -1,15 +1,15 @@
-// Fused HiFi-GAN ResBlock for the narrow stages of the generator (C = 16 / 32 channels), sm_100a.
+// Fused HiFi-GAN ResBlock for the narrow stages of the generator (C = 16 / 32 channels), sm_90a.
 //
 // Reference semantics (models/vocoder/hifigan.py:114-121, one ResBlock with dilations (d0, d1, d2)):
 //     for c1, c2 in zip(convs1, convs2):  xt = c2(lrelu(c1(lrelu(x)))) ;  x = xt + x
 // and the generator's multi-receptive-field sum xs = sum_j resblock_j(x), x = xs / num_kernels (hifigan.py:186-191).
 //
 // Why a dedicated kernel: at C = 16 / 32 a conv run as one GEMM launch moves a 160 MB activation in and two out for a
-// few hundred MFLOP per MB, and a 128 x C output tile lives ~6 us on an SM for ~0.2 us of tensor work
-// (profiles/r01_notes.md).  Here one CTA keeps a time tile of the residual stream in shared memory and runs all six
+// few hundred MFLOP per MB, and a 128 x C output tile holds an SM far longer than its tensor work takes.
+// Here one CTA keeps a time tile of the residual stream in shared memory and runs all six
 // convs of the ResBlock on it; HBM sees the tile once in and once out.  Tap j of a dilated conv is the same smem tile
 // shifted by (j - k/2) * d rows, which ldmatrix addresses directly, so the convs run on mma.sync.m16n8k16 (fp16 in,
-// fp32 accumulate) without any im2col; the tcgen05 path keeps the wide stages (C >= 64) where GEMM tiles are full.
+// fp32 accumulate) without any im2col; the wgmma GEMM keeps the wide stages (C >= 64) where GEMM tiles are full.
 //
 // Rounding points equal the unfused path: every inter-conv activation is rounded to fp16 once (smem), biases and
 // residual adds happen in fp32 before that rounding.  The final (x + res2) * gamma is formed from the fp16 x tile.

@@ -1,9 +1,8 @@
-// Skinny GEMM for the incremental decoder step: out (rows <= 160) x N = A (rows x K) . W^T (N x K), sm_100a.
+// Skinny GEMM for the incremental decoder step: out (rows <= 160) x N = A (rows x K) . W^T (N x K), sm_90a.
 //
 // At 160 rows (32 sentences x beam 5, SURVEY 8a a8) a decoder-layer GEMM streams 2-16 MB of weights for 0.3-2.7 GFLOP:
-// every CTA sees a few dozen KB and the kernel is a single latency chain.  The tcgen05 kernel pays ~9 us per launch for
-// that chain (tensor-map fetch, mbarrier + TMEM setup, TMA round trip, commit, TMEM read-back, staged TMA store,
-// profiles/r01_notes.md).  This kernel does the same product with the shortest chain that still uses tensor cores:
+// every CTA sees a few dozen KB and the kernel is a single latency chain.  The TMA / tensor-core GEMM pays a fixed latency per launch for
+// that chain (tensor-map fetch, mbarrier setup, TMA round trip, MMA group wait, accumulator staging, staged TMA store).  This kernel does the same product with the shortest chain that still uses tensor cores:
 // cp.async straight into padded shared memory (all loads of a CTA in flight at once), ldmatrix + mma.sync.m16n8k16
 // (fp16 in, fp32 accumulate), results stored from registers.  One warp owns one 16-row m-tile and all 64 columns of the
 // CTA's n-tile, so A fragments are read once and the 64-column W tile is shared through smem.

@@ -6,7 +6,7 @@ Reference call stack being replaced: SURVEY.md 3.1 (inference/translator.py:216 
 models/unity/model.py / fairseq2 modules -> models/vocoder/*).
 
 Weight packing (one-time, at load):
-  * Linear weights stay (out,in) fp16 (K-major B operand of the tcgen05 GEMM); biases and LayerNorm params fp32;
+  * Linear weights stay (out,in) fp16 (K-major B operand of the wgmma GEMM); biases and LayerNorm params fp32;
   * q/k/v projections are concatenated into one (3M,M) matrix; cross-attention k/v into (2M,M);
   * Conv1d (out,in,k) -> (out,k,in) so that K index = tap*C_in + c matches the TMA tap walk;
   * GLU-feeding weights are row-interleaved (a_j, b_j) so the GEMM epilogue can gate adjacent accumulator columns;
@@ -76,14 +76,13 @@ class UnitYEngine:
         self.skinny_sites = set(os.environ.get("SB_SKINNY_SITES", "attn").split(","))  # of qkv, attn, ffn1, ffn2
         self.graph_kernels = 0  # kernels executed through CUDA-graph replays (bench.py: gpu_launches)
         # SB_DECODER_FUSED=1: one persistent kernel per decoder step (sb_decoder_step, csrc/decoder_step.cu) instead of the
-        # per-op launch chain.  Opt-in: measured on B200 it is correct and deterministic but not faster (2.6-3.0 ms per step
-        # against 2.3 ms): a grid-wide phase barrier through L2 costs about as much as a kernel boundary inside a CUDA graph
-        # (profiles/r02_notes.md).
+        # per-op launch chain.  Opt-in (correct and deterministic, not timed on H100): a grid-wide phase barrier through L2
+        # costs about as much as a kernel boundary inside a CUDA graph, so the fusion saves launches but not waiting.
         self.decode_fused = os.environ.get("SB_DECODER_FUSED", "0") != "0"
         self.decode_timeline = os.environ.get("SB_DS_TIMELINE", "0") != "0"
-        # SB_DECODE_GEMM_T=1: q|k|v / FFN products of the decoder step on the transposed tcgen05 kernel (decode_gemm.cu).
-        # Opt-in: it moves 2.6x fewer bytes through L2 but measured 12.4 us per launch against 10.7 us for the row-major
-        # kernel at 2 CTAs per SM (profiles/r02_notes.md) - at these sizes the launches are bound by fixed latencies.
+        # SB_DECODE_GEMM_T=1: q|k|v / FFN products of the decoder step on the transposed wgmma kernel (decode_gemm.cu).
+        # Opt-in (not timed on H100): it moves 2.6x fewer bytes through L2, but at these sizes the launches are bound by
+        # fixed latencies rather than by L2 traffic.
         self.decode_gemm_t = os.environ.get("SB_DECODE_GEMM_T", "0") != "0"
         self.topk_tiles = os.environ.get("SB_TOPK_TILES", "1") != "0"  # top-K from the projection's per-tile statistics
 
@@ -431,9 +430,9 @@ class UnitYEngine:
         st["splits_ffn"] = max(1, min(8, k_ffn // 8))
         st["splits_qkv"] = max(1, min(2, k_att // 8))
         # at <= 160 rows the 1024 x 1024 projections of a step (self/cross attention out, cross q) run on the
-        # short-latency mma.sync kernel (skinny_gemm.cu) with more, smaller K slices; measured in-graph on B200
-        # (tools/skinny_bench.py): 4.4 us vs 6.1 us per launch.  The wider products stay on tcgen05 (qkv 8.5 vs 9.8 us,
-        # FFN 11.5 vs 16-20 us: mma.sync runs out of tensor throughput there).  SB_SKINNY_SITES overrides.
+        # short-latency mma.sync kernel (skinny_gemm.cu) with more, smaller K slices (tools/skinny_bench.py times both).
+        # The wider products stay on the wgmma GEMM (mma.sync runs out of tensor throughput there).  SB_SKINNY_SITES
+        # overrides.
         ok = self.decode_skinny and R <= 160 and M % 64 == 0 and c.dec_ffn_dim % 64 == 0
         st["skinny"] = {site: ok and site in self.skinny_sites for site in ("qkv", "attn", "ffn1", "ffn2")}
         sq, sa, sf = self.skinny_splits
@@ -446,7 +445,7 @@ class UnitYEngine:
         while k_att % st["splits_qkv"]: st["splits_qkv"] -= 1
         while k_att % st["splits_attn"]: st["splits_attn"] -= 1
         while k_ffn % st["splits_ffn"]: st["splits_ffn"] -= 1
-        # <= 256 rows: q|k|v, FFN inner and FFN output run on the transposed tcgen05 kernel (decode_gemm.cu: the row-major
+        # <= 256 rows: q|k|v, FFN inner and FFN output run on the transposed wgmma kernel (decode_gemm.cu: the row-major
         # kernel is L2 -> SM bound at these shapes); one (128-feature tile, K slice) unit per CTA, splits fill the machine
         st["gemm_t"] = self.decode_gemm_t and R <= 256 and M % 64 == 0 and c.dec_ffn_dim % 64 == 0
         if st["gemm_t"]:
@@ -511,9 +510,9 @@ class UnitYEngine:
     def _evict_search_states(self, keep):
         """The cache is keyed by problem shape (S_enc and max_len follow the audio length), one entry holds the KV caches,
         the history and two CUDA graphs (~4.8 GB at 32 sentences x beam 5): least-recently-used entries are dropped once
-        the total exceeds SB_SEARCH_CACHE_GB (default 40), so a service fed variable-length audio cannot grow without
+        the total exceeds SB_SEARCH_CACHE_GB (default 24 of an 80 GB device), so a service fed variable-length audio cannot grow without
         bound (the reference frees its search state after every call)."""
-        budget = float(os.environ.get("SB_SEARCH_CACHE_GB", "40")) * 2 ** 30
+        budget = float(os.environ.get("SB_SEARCH_CACHE_GB", "24")) * 2 ** 30
         sizes = {k: self._state_bytes(v) for k, v in self._graphs.items()}
         total = sum(sizes.values())
         for k in list(self._graphs.keys()):
@@ -669,9 +668,9 @@ class UnitYEngine:
 
     def _search_group_count(self, B: int) -> int:
         """Sentences are searched independently (no cross-sentence op, SURVEY 8e), so the batch can be cut into groups
-        whose step chains run concurrently on separate streams.  Measured on B200 at 32 sentences x beam 5 this is
-        slower (232 / 274 / 326 / 368 ms for 1-4 groups: every group re-reads the weights and the chains contend for
-        the same SMs), so the default is one group; SB_SEARCH_GROUPS overrides."""
+        whose step chains run concurrently on separate streams.  Every group re-reads the decoder weights and the chains
+        contend for the same SMs, so the default is one group (more groups are not timed on H100); SB_SEARCH_GROUPS
+        overrides."""
         g = int(os.environ.get("SB_SEARCH_GROUPS", "0")) or self.search_groups
         return max(1, min(g, B // 4)) if B >= 8 else 1
 
@@ -679,8 +678,7 @@ class UnitYEngine:
         """The calling thread's high-priority stream for the search (SB_SEARCH_PRIORITY=1; default off).  The idea: a
         decoder step is a chain of ~260 dependent kernels of a few microseconds, and when other lanes (parallel.LanePool)
         have long GEMM grids of the encoder / T2U / vocoder queued, a high-priority step kernel could take the next free
-        SM slots instead of waiting behind them.  Measured on B200 (profiles/r02_lane_sweep.txt): no difference at 2-4
-        lanes (139 / 152 / 156 utt/s either way), so the search stays on the caller's stream."""
+        SM slots instead of waiting behind them.  Not timed on H100, so the search stays on the caller's stream."""
         if not self.search_priority:
             return None
         s = getattr(self._tls, "hp_stream", None)

@@ -11,7 +11,7 @@ Same inputs and outputs as the reference:
     outputs       <output_path>/<stem>/model-outputs-<stem>.txt  (ref_tgt_text \\t pred_tgt_text [\\t pred_tgt_audio])
                   <output_path>/<stem>/unit_output-<stem>.txt, <output_path>/<stem>/waveform_<stem>/<id>_pred.wav
                   a RuntimeError of predict ("returned no hypothesis") skips the batch                    evaluate.py:293-311
-B200 design instead of the reference's fairseq2 DataPipeline: a small host thread pool decodes audio ahead of the GPU
+design instead of the reference's fairseq2 DataPipeline: a small host thread pool decodes audio ahead of the GPU
 (the reference maps with 4 parallel calls and prefetches 4 batches), the waveforms of a bucket go to the device as one
 padded tensor + lengths, fbank runs there (`Translator.fbank_batch`), and the buckets are spread over
 `parallel.LanePool` lanes so that several batches are in flight per GPU; results are written in file order.

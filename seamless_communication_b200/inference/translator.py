@@ -44,7 +44,7 @@ class Translator:
         self.device = torch.device(device)
         if self.device.type != "cuda":
             # the reference silently switches to fp32 on CPU (translator.py:110-111); this implementation has no CPU path
-            raise RuntimeError("seamless_communication_b200.Translator needs a CUDA device (sm_100a); no CPU fallback exists.")
+            raise RuntimeError("seamless_communication_b200.Translator needs a CUDA device (sm_90a); no CPU fallback exists.")
         if apply_mintox:
             raise NotImplementedError("MinTox re-decoding is outside the S2ST hot path (SURVEY.md 2.1 P14)")
         with_t2u = output_modality != Modality.TEXT  # translator.py:105-107

@@ -116,7 +116,7 @@ def load_unity_model(name_or_arch: str, device="cuda", dtype=torch.float16, stat
     if arch not in cfgmod.UNITY_ARCHS:
         raise ValueError(f"unknown model card / architecture '{name_or_arch}'")
     if dtype != torch.float16:
-        raise ValueError("the sm_100a kernels compute in fp16 with fp32 accumulation; pass dtype=torch.float16")
+        raise ValueError("the sm_90a kernels compute in fp16 with fp32 accumulation; pass dtype=torch.float16")
     cfg = cfgmod.UNITY_ARCHS[arch]()
     if tokenizers is None:
         if not synthetic:

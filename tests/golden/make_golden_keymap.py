@@ -16,6 +16,7 @@ its groups instantiated), plus the entries the function deletes / rewrites.  The
 for the rewritten tensors, checksums - regenerated deterministically by the test from the same seeds."""
 import ast
 import json
+import math
 import os
 import re
 import sys
@@ -90,8 +91,11 @@ def make_inputs(key_map):
 
 
 def checksum(t):
-    t = t.double()
-    return [list(t.shape), float(t.sum()), float((t * torch.arange(1, t.numel() + 1, dtype=torch.float64).view(t.shape)).sum())]
+    # exactly rounded sums (math.fsum; an fp32 value times an index below 2^24 is exact in float64), so the figures do not
+    # depend on the host's reduction order
+    v = t.double().flatten()
+    w = v * torch.arange(1, v.numel() + 1, dtype=torch.float64)
+    return [list(t.shape), math.fsum(v.tolist()), math.fsum(w.tolist())]
 
 
 def main():

@@ -65,12 +65,12 @@ def test_gemm_linear(ops, m, n, k):
 
 
 def test_gemm_wide_tiles_256(ops):
-    """gemm_tc_kernel<256> (two 48 KB stages, 2 CTAs/SM) is selected for fp16 single-output products with n % 256 == 0
-    and >= 296 tiles - the encoder / T2U / vocoder shapes: every epilogue it serves against fp32 torch (bias, SiLU, GLU,
+    """gemm_tc_kernel<256> (three 48 KB stages, 1 CTA/SM) is selected for fp16 single-output products with n % 256 == 0
+    and at least two tiles per SM (264 on an H100) - the encoder / T2U / vocoder shapes: every epilogue it serves against fp32 torch (bias, SiLU, GLU,
     residual + scales, conv taps over a ragged sequence batch with zeroed padding)."""
     from seamless_communication_b200.ops import Seq
     torch.manual_seed(256)
-    m, k = 10000, 320  # 79 M tiles x (n / 256) >= 296 for n >= 1024
+    m, k = 10000, 320  # 79 M tiles x (n / 256) >= 316 tiles for n >= 1024: at least two per SM up to 158 SMs
     a = (torch.randn(m, k, device=dev) * 0.5).half()
     for n in (1024, 1280):
         w = (torch.randn(n, k, device=dev) * 0.05).half()
@@ -152,7 +152,7 @@ def test_gemm_skinny_matches_simt_reference(ops, rows, n, k, splits):
     out.buf.fill_(float("nan"))
     ops.gemm_skinny(a, w, n, bias, act=ops.ACT_RELU, out=out)
     assert (out.buf.float() - want).abs().max() < 4e-3  # + fp16 rounding of the output
-    # same partials as the tcgen05 split-K kernel up to fp32 summation order
+    # same partials as the wgmma split-K kernel up to fp32 summation order
     part2 = torch.zeros((splits * SR, n), device=dev)
     ops.gemm_splitk(a, w, n, splits, part2)
     assert (part2.view(splits, SR, n)[:, :rows].sum(0) + bias - got).abs().max() < 1e-3
@@ -161,7 +161,7 @@ def test_gemm_skinny_matches_simt_reference(ops, rows, n, k, splits):
 @pytest.mark.parametrize("rows,n,k,splits", [(160, 3072, 1024, 6), (160, 1024, 8192, 16), (160, 8192, 1024, 1), (40, 384, 128, 2),
                                              (5, 256, 128, 1), (256, 200, 192, 3), (33, 1126, 128, 1)])
 def test_gemm_decode_transposed_matches_simt_reference(ops, rows, n, k, splits):
-    """decode_gemm.cu (weights as the tcgen05 A operand, all rows as B): split-K partials sum to the product (uneven K
+    """decode_gemm.cu (weights as the wgmma A operand, all rows as B): split-K partials sum to the product (uneven K
     slices, ragged last feature tile, rows that are not a multiple of 16), and the direct mode applies bias + ReLU; both
     against the CUDA-core reference kernel."""
     from seamless_communication_b200.ops import Seq
@@ -865,13 +865,24 @@ def test_full_width_s2st_matches_oracle(base, ops):
     assert ulens.tolist() == ref["unit_lens"].tolist()
     n = int(ref["unit_lens"][0])
     assert n == 495  # 99 subwords x 5 characters, duration 1 each (SURVEY 8d)
-    diff = int((units[0, :n].cpu() != ref["units"][0, :n]).sum())
-    assert diff <= 1, f"{diff} unit ids differ from the oracle"
+    pos = (units[0, :n].cpu() != ref["units"][0, :n]).nonzero().flatten().tolist()
+    diff = len(pos)
+    # margin audit, as for the search above: a differing unit is an fp16 argmax near tie only if it is the oracle's own
+    # runner-up and the oracle's fp32 top-2 margin there is below one fp16 step at that position's top logit
+    top2 = ref["logits"][0].float()[pos].topk(2, dim=-1) if pos else None
+
+    def fp16_step(x):  # spacing of fp16 values around x (subnormal spacing below 2^-14)
+        return 2.0 ** max(math.frexp(abs(x))[1] - 11, -24)
+
+    ties = [i for i, p in enumerate(pos)
+            if float(top2.values[i, 0] - top2.values[i, 1]) < fp16_step(float(top2.values[i, 0]))
+            and int(units[0, p]) - int(ref["units"][0, p]) == int(top2.indices[i, 1]) - int(top2.indices[i, 0])]
+    assert diff - len(ties) <= 1, f"{diff} unit ids differ from the oracle, {len(ties)} of them near ties"
     # --- a15/a16: waveform from the oracle's units, and the trimming rule
     wav = voc(ref["units"].to(dev), "spa", -1, dur_prediction=False)
     err_wav = (wav.float().cpu() - ref["wav_full"]).abs().max().item()
     assert err_wav < 5e-3, f"waveform abs err {err_wav}"
-    print(f"full width: enc {err_enc:.1e} dec {err_dec:.1e} logits {err_lg:.1e} units diff {diff} wav {err_wav:.1e} "
+    print(f"full width: enc {err_enc:.1e} dec {err_dec:.1e} logits {err_lg:.1e} units diff {diff} ({len(ties)} near ties) wav {err_wav:.1e} "
           f"search common prefix {same_prefix}/{len(ids)}")
 
 

@@ -1,5 +1,5 @@
 import sys, torch, os
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from seamless_communication_b200 import ops
 from seamless_communication_b200.ops import Seq
 torch.manual_seed(0)

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Staged bring-up checks on a real B200 (development aid; the judged tests live in tests/).
+"""Staged bring-up checks on a real H100 (development aid; the tests live in tests/).
 Usage: python tools/gpu_check.py [stage ...]   stages: gemm fbank ln attn dwconv encoder decode t2u vocoder e2e"""
 import os
 import sys

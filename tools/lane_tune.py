@@ -1,4 +1,4 @@
-"""Decoder-step kernel choices (skinny sites / split counts / transposed tcgen05 / L2 prefetch) timed with 1 and with
+"""Decoder-step kernel choices (skinny sites / split counts / transposed wgmma / L2 prefetch) timed with 1 and with
 `--lanes` beam searches in flight: under lanes the cheapest choice in SM-slot time wins, not the shortest latency chain.
 Usage: python tools/lane_tune.py [--lanes 4]"""
 import argparse

@@ -1,13 +1,13 @@
 """Per-kernel ncu summary of one S2ST step and the DRAM traffic of one beam-search step.
 
-On the GPU box (one GPU, under gpurun):
+On a machine with the GPU and Nsight Compute:
     SB_BENCH_HARD_MAX=14 ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum,\
 sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active --clock-control none --csv \
-        --log-file gpurun_out/r02_step_metrics.csv python bench.py --profile-only
-Here (no GPU):
-    python tools/ncu_summary.py gpurun_out/r02_step_metrics.csv --hard-max 14
-writes profiles/r02_kernels_ncu.txt (one line per kernel: launches, mean / total duration, share of the step, DRAM bytes
-per launch, achieved GB/s, tensor-pipe %) and profiles/r02_decode_step_dram.json (bench.py reads it for roofline.traffic).
+        --log-file step_metrics.csv python bench.py --profile-only
+Anywhere:
+    python tools/ncu_summary.py step_metrics.csv --hard-max 14
+writes profiles/<tag>_kernels_ncu.txt (one line per kernel: launches, mean / total duration, share of the step, DRAM bytes
+per launch, achieved GB/s, tensor-pipe %) and profiles/<tag>_decode_step_dram.json (DRAM bytes per beam-search step).
 Per-launch times under ncu are cold-cache and serialised: the SHARES are what to compare."""
 import argparse
 import collections

@@ -46,9 +46,9 @@ def main():
     def kinds(d):
         st = lambda: torch.cuda.current_stream().cuda_stream  # noqa: E731
         return {
-            "qkv  tcgen05 split 2": lambda: ops.gemm_splitk(d["h"], w_qkv, 3 * M, 2, d["part_qkv"]),
-            "ffn1 tcgen05 direct": lambda: ops.gemm(d["h"], w_1, F, b_f, act=ACT_RELU, out=d["ffn"]),
-            "ffn2 tcgen05 split 8": lambda: ops.gemm_splitk(d["ffn"], w_2, M, 8, d["part"]),
+            "qkv  wgmma split 2": lambda: ops.gemm_splitk(d["h"], w_qkv, 3 * M, 2, d["part_qkv"]),
+            "ffn1 wgmma direct": lambda: ops.gemm(d["h"], w_1, F, b_f, act=ACT_RELU, out=d["ffn"]),
+            "ffn2 wgmma split 8": lambda: ops.gemm_splitk(d["ffn"], w_2, M, 8, d["part"]),
             "out  skinny split 8": lambda: ops.gemm_splitk(d["att"], w_o, M, 8, d["part"], skinny=True),
             "qkv  skinny split 4": lambda: ops.gemm_splitk(d["h"], w_qkv, 3 * M, 4, d["part_qkv"], skinny=True),
             "ffn2 skinny split 16": lambda: ops.gemm_splitk(d["ffn"], w_2, M, 16, d["part"], skinny=True),

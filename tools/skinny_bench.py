@@ -1,4 +1,4 @@
-"""In-graph time per launch of the decoder-step GEMMs (160 rows): tcgen05 split-K kernel vs the mma.sync skinny kernel.
+"""In-graph time per launch of the decoder-step GEMMs (160 rows): wgmma split-K kernel vs the mma.sync skinny kernel.
 Each graph chains 96 launches over 24 different weight tensors (a decoder step never re-reads a weight from L2)."""
 import os, sys, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
