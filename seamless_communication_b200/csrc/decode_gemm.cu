@@ -3,8 +3,8 @@
 // At 160 rows the general kernel (gemm_tcgen05.cu: rows = MMA M, 64 output features per CTA) is bound by L2 -> SM traffic, not
 // by HBM: every CTA re-reads its 128-row activation tile for each of its few weight rows.  Here a 128-FEATURE weight tile is
 // the wgmma A operand (two consumer warpgroups, 64 features each) and ALL rows are the B operand (N = rows padded to a
-// power of two >= 32, fp32 accumulators in registers): a CTA reads its weight tile once and the activations once per
-// k-block.  One (tile, K-slice) unit per CTA, a deep TMA ring (the unit is a chain of k-blocks), one producer warp.
+// power of two >= 32, or to 160 for a beam-search step of 32 x 5 rows; fp32 accumulators in registers): a CTA reads its
+// weight tile once and the activations once per k-block.  One (tile, K-slice) unit per CTA, a deep TMA ring (the unit is a chain of k-blocks), one producer warp.
 //   split-K mode : slice z writes raw fp32 partial products to partials[(z * slice_rows + row) * n + feature]
 //                  (same contract as sb_gemm_splitk / sb_gemm_skinny; reduced by sb_splitk_reduce_ln or the attention kernels)
 //   direct mode  : out[row * out_ld + feature] = act(acc + bias) in fp16, act in {none, relu}
@@ -208,7 +208,7 @@ extern "C" int sb_gemm_decode(const sb_gemm_t* g, int32_t splits, float* partial
   a.out_ld = g->out_ld;
   a.prefetch = (const char*)g->prefetch;
   a.prefetch_bytes = g->prefetch ? g->prefetch_bytes / 4096 * 4096 : 0;
-  const int nt = a.npad <= 32 ? 32 : a.npad <= 64 ? 64 : a.npad <= 128 ? 128 : 256;
+  const int nt = a.npad <= 32 ? 32 : a.npad <= 64 ? 64 : a.npad <= 128 ? 128 : a.npad <= 160 ? 160 : 256;
   const int stage_bytes = DG_W_BYTES + nt * DG_BK * 2;
   int dev = 0, smem_optin = 0;
   SB_CUDA_OK(cudaGetDevice(&dev));
@@ -231,5 +231,6 @@ extern "C" int sb_gemm_decode(const sb_gemm_t* g, int32_t splits, float* partial
   if (nt == 32) return dg_launch<32>(tmW, tmX, a, grid, smem, st);
   if (nt == 64) return dg_launch<64>(tmW, tmX, a, grid, smem, st);
   if (nt == 128) return dg_launch<128>(tmW, tmX, a, grid, smem, st);
+  if (nt == 160) return dg_launch<160>(tmW, tmX, a, grid, smem, st);
   return dg_launch<256>(tmW, tmX, a, grid, smem, st);
 }

@@ -75,12 +75,6 @@ struct TileCfg {
   static_assert(BN >= 256 || OUT2_OFFSET + (BN / 64 > 0 ? BN / 64 : 1) * 16384 <= STAGES * STAGE_BYTES, "staging does not fit");
 };
 
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, const void* smem_src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
-}
-
 __device__ unsigned long long* g_timeline = nullptr;
 __device__ __forceinline__ unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
 #define TL(i) do { if (g_timeline != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0) g_timeline[i] = gtime(); } while (0)
@@ -427,8 +421,8 @@ static EncodeTiledFn get_encode_fn() {
 }
 
 // 2D tensor (inner = channels, outer = rows), box box_cols x box_rows (box_cols * esize = 128 B), 128B swizzle, OOB -> 0
-static int make_tmap(CUtensorMap* tm, const void* base, uint64_t inner, uint64_t rows, uint64_t ld_elems,
-                     uint32_t box_rows, int esize = 2) {
+int make_tmap(CUtensorMap* tm, const void* base, uint64_t inner, uint64_t rows, uint64_t ld_elems, uint32_t box_rows,
+              int esize) {
   EncodeTiledFn fn = get_encode_fn();
   SB_REQUIRE(fn != nullptr, SB_ECUDA, "cuTensorMapEncodeTiled entry point not available");
   cuuint64_t dims[2] = {inner, rows};
@@ -613,6 +607,10 @@ extern "C" int sb_gemm(const sb_gemm_t* g_in, sb_stream_t stream) {
   auto tiles = [&](int bn) { return mt * ((g->n + bn - 1) / bn); };
   if (g->tile_stats != nullptr) {
     SB_REQUIRE(!g->glu && g->n >= 128, SB_ENOSUP, "sb_gemm: tile_stats needs n >= 128 and no GLU");
+    // up to 256 rows (a beam-search step): the weight-stationary kernel of vocab_proj.cu, which reads each weight row once.
+    // SB_PROJ_T=0 selects the general kernel (read per call: tools compare both inside one process)
+    const char* ep = getenv("SB_PROJ_T");
+    if ((ep == nullptr || atoi(ep) != 0) && sb::vocab_proj_supported(g)) return sb::vocab_proj(g, st);
     return sb::launch<128>(g, st);  // the statistics are per 128-column tile (SB_STATS_TILE)
   }
   // 256-wide tiles for the large products (encoder / T2U / vocoder GEMMs): fp16 single-output epilogues, whole tiles only
