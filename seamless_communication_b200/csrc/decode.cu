@@ -881,6 +881,16 @@ extern "C" int sb_embed_seq(const int32_t* ids, int32_t ids_ld, int32_t L, const
   return SB_OK;
 }
 
+// A launch whose dynamic plus static shared memory exceeds 48 KB needs the kernel's opt-in attribute (set per device, so
+// it is set on every such launch; the self-attention kernels hold 1.5 KB of static staging next to their dynamic scratch)
+template <typename Kernel>
+static cudaError_t allow_dynamic_smem(Kernel kernel, size_t dyn) {
+  cudaFuncAttributes a;
+  cudaError_t e = cudaFuncGetAttributes(&a, kernel);
+  if (e != cudaSuccess || dyn + a.sharedSizeBytes <= 48 * 1024) return e;
+  return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
+}
+
 extern "C" int sb_decode_self_attn(const void* qkv, const float* qkv_partials, int32_t splits, int64_t slice_rows,
                                    const float* qkv_bias, void* kcache, void* vcache, const int32_t* anc, int32_t anc_ld,
                                    const int32_t* step_ptr, int32_t max_len, void* out, int32_t rows, int32_t heads,
@@ -892,6 +902,7 @@ extern "C" int sb_decode_self_attn(const void* qkv, const float* qkv_partials, i
   static int v2 = -1;
   if (v2 < 0) { const char* e = getenv("SB_SELF_ATTN_V2"); v2 = (e == nullptr || atoi(e) != 0) ? 1 : 0; }
   if (v2 && qkv == nullptr && (size_t)4 * max_len * sizeof(int) <= 48 * 1024) {
+    if (max_len > 2048) SB_CUDA_OK(allow_dynamic_smem(decode_self_attn2_kernel, (size_t)4 * max_len * sizeof(int)));
     SB_CUDA_OK(launch_k(decode_self_attn2_kernel, dim3(rows, (heads + 3) / 4), dim3(128), (size_t)4 * max_len * sizeof(int),
                          (cudaStream_t)stream, qkv_partials, (int)splits, (long long)slice_rows, qkv_bias, (elem_t*)kcache, (elem_t*)vcache,
                          (const int*)anc, (int)anc_ld, (const int*)step_ptr, (int)max_len, (elem_t*)out, (int)rows, (int)heads));
@@ -900,6 +911,7 @@ extern "C" int sb_decode_self_attn(const void* qkv, const float* qkv_partials, i
   }
   size_t smem = (size_t)8 * max_len * sizeof(float);
   SB_REQUIRE(smem <= 48 * 1024, SB_ENOSUP, "sb_decode_self_attn: max_len %d too large", max_len);
+  if (max_len > 1024) SB_CUDA_OK(allow_dynamic_smem(decode_self_attn_kernel, smem));
   SB_CUDA_OK(launch_k(decode_self_attn_kernel, dim3(rows, (heads + 3) / 4), dim3(128), smem, (cudaStream_t)stream,
                        (const elem_t*)qkv, qkv_partials, (int)splits, (long long)slice_rows, qkv_bias, (elem_t*)kcache,
                        (elem_t*)vcache, (const int*)anc, (int)anc_ld, (const int*)step_ptr,

@@ -402,7 +402,7 @@ class UnitYEngine:
         """Static buffers + captured CUDA graphs of one decoder step, cached per problem shape so that repeated
         predict() calls replay the same graphs (the reference rebuilds its generator per call, translator.py:179-186;
         construction here stays cheap after the first call)."""
-        key = (B, S_enc, ML, beam, P, has_lens, use_graph, slot, self.decode_fused, self.lane)
+        key = (B, S_enc, ML, beam, P, has_lens, use_graph, slot, self.decode_fused, self.decode_gemm_t, self.lane)
         st = self._graphs.get(key)
         if st is not None:
             self._graphs.move_to_end(key)
@@ -713,6 +713,9 @@ class UnitYEngine:
         ML = hard_max if a <= 0 else min(hard_max, int(a * S_enc) + b)  # fairseq2.cpp:1097-1105
         P = len(prefix)
         assert 1 <= P < ML
+        if ML > self.cfg.max_seq_len:  # fairseq2's position encoder raises here; embed_kernel would read past the sinusoid table
+            raise ValueError(f"The input sequence length must be less than or equal to the maximum sequence length "
+                             f"({self.cfg.max_seq_len}), but is {ML} instead.")
         assert enc.PH == 0 and enc.Tp == enc.T, "encoder output must be a halo-free Seq"
         G = self._search_group_count(B)
         bounds = [(B * g) // G for g in range(G + 1)]
