@@ -319,7 +319,9 @@ int sb_vocoder_embed(const int32_t* units, int32_t U, int32_t batch, const void*
  *   out  = (resblock(x) + res2) * gamma        res2 = running sum over the generator's ResBlocks or NULL
  *   out2 = leaky_relu(out, out2_slope)         optional (the activation that feeds the next stage, hifigan.py:183/192)
  * Weights are the folded weight-norm kernels in sb_gemm conv layout (C, kernel_size * C), biases fp32.
- * Every row of `out` / `out2` that belongs to a sequence or its halo is written (halo rows with zeros). */
+ * Every row of `out` / `out2` that belongs to a sequence or its halo is written (halo rows with zeros).
+ * lens (optional, int32 [batch], each <= T): sequence b has lens[b] rows; every conv sees rows >= lens[b] as zero
+ * padding, as it would for that sequence alone, and those rows of `out` / `out2` are written as 0. */
 typedef struct {
   const void* x; const void* res2; void* out; void* out2;
   const void* w1[3]; const float* b1[3];   /* convs1: dilation[i] */
@@ -329,10 +331,12 @@ typedef struct {
   int32_t batch, T, rows_per_seq, halo;    /* sequence layout: data rows [halo, halo + T) of each rows_per_seq block */
   float slope;                             /* leaky-relu slope inside the block (hifigan.py:12 LRELU_SLOPE) */
   float gamma, out2_slope;
+  const int32_t* lens;                     /* optional per-sequence lengths (NULL: every sequence has T rows) */
 } sb_resblock_t;
 int sb_hifigan_resblock(const sb_resblock_t* r, sb_stream_t stream);
-/* final conv_post (C->1, k7) + tanh on CUDA cores: wav fp32 [B][T] from lrelu'ed activations in sequence layout */
-int sb_conv_post_tanh(const void* x, int32_t x_rows, int32_t x_halo, int32_t T, int32_t C, int32_t batch,
+/* final conv_post (C->1, k7) + tanh on CUDA cores: wav fp32 [B][T] from lrelu'ed activations in sequence layout;
+ * lens (optional, int32 [B]): wav[b][t] = 0 for t >= lens[b] */
+int sb_conv_post_tanh(const void* x, int32_t x_rows, int32_t x_halo, int32_t T, const int32_t* lens, int32_t C, int32_t batch,
                       const void* w, float bias, int32_t k, float* wav, int64_t wav_ld, sb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------

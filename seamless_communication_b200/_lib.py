@@ -33,7 +33,7 @@ class ResblockDesc(C.Structure):
         ("w1", c_p * 3), ("b1", c_p * 3), ("w2", c_p * 3), ("b2", c_p * 3),
         ("dilation", i32 * 3), ("channels", i32), ("kernel_size", i32),
         ("batch", i32), ("T", i32), ("rows_per_seq", i32), ("halo", i32),
-        ("slope", f32), ("gamma", f32), ("out2_slope", f32),
+        ("slope", f32), ("gamma", f32), ("out2_slope", f32), ("lens", c_p),
     ]
 
 
@@ -117,7 +117,7 @@ PROTOTYPES = {
     "sb_unit_argmax": [c_p, i64, i32, i32, i32, i32, i32, c_p, i32, i32, c_p, c_p],
     "sb_hifigan_resblock": [c_p, c_p],
     "sb_vocoder_embed": [c_p, i32, i32, c_p, i32, c_p, i32, c_p, c_p, i32, c_p, c_p, i32, i32, c_p],
-    "sb_conv_post_tanh": [c_p, i32, i32, i32, i32, i32, c_p, f32, i32, c_p, i64, c_p],
+    "sb_conv_post_tanh": [c_p, i32, i32, i32, c_p, i32, i32, c_p, f32, i32, c_p, i64, c_p],
     "sb_avgpool_time": [c_p, c_p, i32, i32, i32, i32, c_p],
     "sb_pchoose": [c_p, c_p, c_p, i32, i32, i32, f32, f32, c_p],
     "sb_cast_f32_to_f16": [c_p, c_p, i64, c_p],

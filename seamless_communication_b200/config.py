@@ -117,6 +117,9 @@ class VocoderConfig:
     num_langs: int = 36
     spkr_embedding_dim: int = 256
     num_spkrs: int = 200
+    # duration predictor (dur_predictor_params of builder.py:53-58): VariancePredictor over the unit embeddings
+    var_pred_hidden: int = 1280
+    var_pred_kernel: int = 3
     langs: Tuple[str, ...] = VOCODER_LANGS_V2
 
     @property
@@ -186,6 +189,7 @@ def tiny_vocoder() -> VocoderConfig:
         embedding_dim=64,
         lang_embedding_dim=32,
         spkr_embedding_dim=32,
+        var_pred_hidden=64,
     )
 
 

@@ -37,6 +37,7 @@ struct ResblockArgs {
   int dil[3];
   int k, T, Tp, PH;
   float slope, gamma, out2_slope;
+  const int* lens;     // optional per-sequence lengths (<= T); rows past them are zero padding and are written as 0
 };
 
 template <int C>
@@ -157,52 +158,59 @@ __global__ void __launch_bounds__(RB_THREADS, C == 16 ? 2 : 1) resblock_kernel(c
   const int t_first = blockIdx.x * TT - H;                   // time index of tile row 0
   const long long seq0 = ((long long)b * p.Tp + p.PH) * C;   // element offset of (b, t = 0)
   pdl_sync();
-  // guard rows (never part of a valid output's receptive field, zeroed so that no NaN pattern is ever multiplied)
-  for (int i = threadIdx.x; i < RB_GUARD * LD / 8 * 2; i += RB_THREADS) {
-    const int side = i / (RB_GUARD * LD / 8), j = i - side * (RB_GUARD * LD / 8);
-    const int off = (side ? (RB_GUARD + RB_ROWS) * LD : 0) + j * 8;
-    const uint4 z = make_uint4(0, 0, 0, 0);
-    *reinterpret_cast<uint4*>(as + off) = z;
-    *reinterpret_cast<uint4*>(ts + off) = z;
-  }
-  // tile load: x and lrelu(x); rows outside [0, T) are zero
-  for (int i = threadIdx.x; i < RB_ROWS * VEC; i += RB_THREADS) {
-    const int r = i / VEC, v = i - r * VEC;
-    const int t = t_first + r;
-    uint4 u = make_uint4(0, 0, 0, 0);
-    if (t >= 0 && t < p.T) u = *reinterpret_cast<const uint4*>(p.x + seq0 + (long long)t * C + v * 8);
-    uint4 a;
-    const __half2* h = reinterpret_cast<const __half2*>(&u);
-    __half2* ha = reinterpret_cast<__half2*>(&a);
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const float2 f = __half22float2(h[e]);
-      ha[e] = __floats2half2_rn(rb_lrelu(f.x, p.slope), rb_lrelu(f.y, p.slope));
+  const int Tb = p.lens != nullptr ? min(p.lens[b], p.T) : p.T;  // this sequence's length
+  // a tile whose valid outputs all lie past Tb only writes zeros
+  const bool idle = blockIdx.x * TT >= Tb;
+  if (!idle) {
+    // guard rows (never part of a valid output's receptive field, zeroed so that no NaN pattern is ever multiplied)
+    for (int i = threadIdx.x; i < RB_GUARD * LD / 8 * 2; i += RB_THREADS) {
+      const int side = i / (RB_GUARD * LD / 8), j = i - side * (RB_GUARD * LD / 8);
+      const int off = (side ? (RB_GUARD + RB_ROWS) * LD : 0) + j * 8;
+      const uint4 z = make_uint4(0, 0, 0, 0);
+      *reinterpret_cast<uint4*>(as + off) = z;
+      *reinterpret_cast<uint4*>(ts + off) = z;
     }
-    const int off = (RB_GUARD + r) * LD + v * 8;
-    *reinterpret_cast<uint4*>(xs + off) = u;
-    *reinterpret_cast<uint4*>(as + off) = a;
-  }
+    // tile load: x and lrelu(x); rows outside [0, Tb) are zero
+    for (int i = threadIdx.x; i < RB_ROWS * VEC; i += RB_THREADS) {
+      const int r = i / VEC, v = i - r * VEC;
+      const int t = t_first + r;
+      uint4 u = make_uint4(0, 0, 0, 0);
+      if (t >= 0 && t < Tb) u = *reinterpret_cast<const uint4*>(p.x + seq0 + (long long)t * C + v * 8);
+      uint4 a;
+      const __half2* h = reinterpret_cast<const __half2*>(&u);
+      __half2* ha = reinterpret_cast<__half2*>(&a);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float2 f = __half22float2(h[e]);
+        ha[e] = __floats2half2_rn(rb_lrelu(f.x, p.slope), rb_lrelu(f.y, p.slope));
+      }
+      const int off = (RB_GUARD + r) * LD + v * 8;
+      *reinterpret_cast<uint4*>(xs + off) = u;
+      *reinterpret_cast<uint4*>(as + off) = a;
+    }
 #pragma unroll 1
-  for (int pair = 0; pair < 3; ++pair) {
-    rb_load_weights<C>(ws, p.w1[pair], p.k);
-    __syncthreads();  // weights + the previous stage's activations are in place
-    rb_conv<C, false>(as, xs, as, ts, ws, p.b1[pair], p.k, p.dil[pair], t_first, p.T, p.slope);
-    __syncthreads();  // ts complete, ws free
-    rb_load_weights<C>(ws, p.w2[pair], p.k);
-    __syncthreads();
-    rb_conv<C, true>(ts, xs, as, ts, ws, p.b2[pair], p.k, 1, t_first, p.T, p.slope);
-    __syncthreads();  // xs / as complete, ws free
+    for (int pair = 0; pair < 3; ++pair) {
+      rb_load_weights<C>(ws, p.w1[pair], p.k);
+      __syncthreads();  // weights + the previous stage's activations are in place
+      rb_conv<C, false>(as, xs, as, ts, ws, p.b1[pair], p.k, p.dil[pair], t_first, Tb, p.slope);
+      __syncthreads();  // ts complete, ws free
+      rb_load_weights<C>(ws, p.w2[pair], p.k);
+      __syncthreads();
+      rb_conv<C, true>(ts, xs, as, ts, ws, p.b2[pair], p.k, 1, t_first, Tb, p.slope);
+      __syncthreads();  // xs / as complete, ws free
+    }
   }
-  // write the valid rows: out = (x + res2) * gamma, out2 = lrelu(out)
+  // write the valid rows: out = (x + res2) * gamma, out2 = lrelu(out); rows in [Tb, T) get zeros
   for (int i = threadIdx.x; i < TT * VEC; i += RB_THREADS) {
     const int rr = i / VEC, v = i - rr * VEC;
     const int r = H + rr, t = t_first + r;
     if (t >= p.T) continue;
     const long long g = seq0 + (long long)t * C + v * 8;
-    const uint4 u = *reinterpret_cast<const uint4*>(xs + (RB_GUARD + r) * LD + v * 8);
+    const bool live = t < Tb;
+    uint4 u = make_uint4(0, 0, 0, 0);
+    if (live) u = *reinterpret_cast<const uint4*>(xs + (RB_GUARD + r) * LD + v * 8);
     uint4 rz = make_uint4(0, 0, 0, 0);
-    if (p.res2 != nullptr) rz = *reinterpret_cast<const uint4*>(p.res2 + g);
+    if (p.res2 != nullptr && live) rz = *reinterpret_cast<const uint4*>(p.res2 + g);
     const __half2* h = reinterpret_cast<const __half2*>(&u);
     const __half2* hr = reinterpret_cast<const __half2*>(&rz);
     uint4 o, o2;
@@ -279,6 +287,7 @@ extern "C" int sb_hifigan_resblock(const sb_resblock_t* r, sb_stream_t stream) {
   a.out = (sb::elem_t*)r->out; a.out2 = (sb::elem_t*)r->out2;
   a.k = r->kernel_size; a.T = r->T; a.Tp = r->rows_per_seq; a.PH = r->halo;
   a.slope = r->slope; a.gamma = r->gamma; a.out2_slope = r->out2_slope;
+  a.lens = r->lens;
   cudaStream_t st = (cudaStream_t)stream;
   return r->channels == 16 ? sb::launch_resblock<16>(a, r->batch, st) : sb::launch_resblock<32>(a, r->batch, st);
 }

@@ -27,16 +27,21 @@ __global__ void __launch_bounds__(256) vocoder_embed_kernel(const int* __restric
   }
 }
 
-// wav[b][t] = tanh(bias + sum_{j,c} x[b][t + j - k/2][c] * w[j][c]);  x is already leaky-relu'ed, halos are zero
-__global__ void __launch_bounds__(256) conv_post_tanh_kernel(const elem_t* __restrict__ x, int x_rows, int x_halo, int T, int C,
-                                                             const elem_t* __restrict__ w, float bias, int k,
-                                                             float* __restrict__ wav, long long wav_ld) {
+// wav[b][t] = tanh(bias + sum_{j,c} x[b][t + j - k/2][c] * w[j][c]);  x is already leaky-relu'ed, halos are zero.
+// With per-sequence lengths, wav[b][t] = 0 for t >= lens[b].
+__global__ void __launch_bounds__(256) conv_post_tanh_kernel(const elem_t* __restrict__ x, int x_rows, int x_halo, int T,
+                                                             const int* __restrict__ lens, int C, const elem_t* __restrict__ w,
+                                                             float bias, int k, float* __restrict__ wav, long long wav_ld) {
   extern __shared__ float sw[];  // [k*C]
   for (int i = threadIdx.x; i < k * C; i += blockDim.x) sw[i] = __half2float(w[i]);
   __syncthreads();
   const int b = blockIdx.y;
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= T) return;
+  if (lens != nullptr && t >= lens[b]) {
+    wav[(long long)b * wav_ld + t] = 0.f;
+    return;
+  }
   const elem_t* xp = x + ((long long)b * x_rows + x_halo + t - k / 2) * C;  // halo >= k/2 guarantees in-bounds zeros
   float acc = bias;
   for (int i = 0; i < k * C; i += 8) {
@@ -65,14 +70,15 @@ extern "C" int sb_vocoder_embed(const int32_t* units, int32_t U, int32_t batch, 
   return SB_OK;
 }
 
-extern "C" int sb_conv_post_tanh(const void* x, int32_t x_rows, int32_t x_halo, int32_t T, int32_t C, int32_t batch, const void* w,
-                                 float bias, int32_t k, float* wav, int64_t wav_ld, sb_stream_t stream) {
+extern "C" int sb_conv_post_tanh(const void* x, int32_t x_rows, int32_t x_halo, int32_t T, const int32_t* lens, int32_t C,
+                                 int32_t batch, const void* w, float bias, int32_t k, float* wav, int64_t wav_ld,
+                                 sb_stream_t stream) {
   using namespace sb;
   SB_REQUIRE(x && w && wav && T > 0 && batch > 0 && k > 0, SB_EINVAL, "sb_conv_post_tanh: bad args");
   SB_REQUIRE(C % 8 == 0 && x_halo >= k / 2, SB_ENOSUP, "sb_conv_post_tanh: C must be a multiple of 8 and halo >= k/2");
   dim3 grid((T + 255) / 256, batch);
-  conv_post_tanh_kernel<<<grid, 256, (size_t)k * C * sizeof(float), (cudaStream_t)stream>>>((const elem_t*)x, x_rows, x_halo, T, C,
-                                                                                          (const elem_t*)w, bias, k, wav, wav_ld);
+  conv_post_tanh_kernel<<<grid, 256, (size_t)k * C * sizeof(float), (cudaStream_t)stream>>>((const elem_t*)x, x_rows, x_halo, T, lens,
+                                                                                          C, (const elem_t*)w, bias, k, wav, wav_ld);
   SB_LAUNCH_OK();
   return SB_OK;
 }

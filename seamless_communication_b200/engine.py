@@ -906,7 +906,16 @@ class VocoderEngine:
 
     HALO0 = 5  # unit-rate halo; scales with the upsampling so that stage 1 has the 25 rows k=11,d=5 needs
 
+    DUR_PREDICTOR_KEYS = tuple("code_generator.dur_predictor." + n for n in (
+        "conv1.0.weight", "conv1.0.bias", "ln1.weight", "ln1.bias", "conv2.0.weight", "conv2.0.bias", "ln2.weight",
+        "ln2.bias", "proj.weight", "proj.bias"))
+
     def __init__(self, cfg: VocoderConfig, state_dict: Dict[str, torch.Tensor], device="cuda"):
+        # the duration predictor is optional, as in the reference (codehifigan.py:45-47): all of its tensors or none
+        missing = [k for k in self.DUR_PREDICTOR_KEYS if k not in state_dict]
+        if 0 < len(missing) < len(self.DUR_PREDICTOR_KEYS):
+            raise ValueError(f"incomplete vocoder duration predictor: missing {missing}")
+        self.has_dur_predictor = not missing
         _lib.require_cuda()
         self.cfg, self.device = cfg, torch.device(device)
         self.fused_resblocks = os.environ.get("SB_FUSED_RESBLOCK", "1") != "0"  # 16/32-channel stages: resblock.cu
@@ -949,17 +958,95 @@ class VocoderEngine:
         cp = folded("conv_post")  # (1, C, 7)
         w["conv_post.w"] = cp.permute(0, 2, 1).reshape(-1).to(dev, F16).contiguous()
         self.conv_post_bias = float(sd[P + "conv_post.bias"][0])
+        if self.has_dur_predictor:
+            dp = "dur_predictor."
+            H, K = c.var_pred_hidden, c.var_pred_kernel
+            for name, cin in (("conv1.0", c.embedding_dim), ("conv2.0", H)):
+                cw = sd[P + dp + name + ".weight"]
+                if tuple(cw.shape) != (H, cin, K) or K % 2 == 0:
+                    raise ValueError(f"{P}{dp}{name}.weight has shape {tuple(cw.shape)}, expected ({H}, {cin}, {K}) "
+                                     f"with an odd kernel")
+                w[dp + name + ".w"] = cw.permute(0, 2, 1).reshape(H, -1).to(dev, F16).contiguous()  # (out, k, in)
+                w[dp + name + ".b"] = sd[P + dp + name + ".bias"].to(dev, torch.float32).contiguous()
+            for name in ("ln1", "ln2"):
+                w[dp + name + ".w"] = sd[P + dp + name + ".weight"].to(dev, torch.float32).contiguous()
+                w[dp + name + ".b"] = sd[P + dp + name + ".bias"].to(dev, torch.float32).contiguous()
+            w[dp + "proj.w"] = sd[P + dp + "proj.weight"].reshape(-1).to(dev, F16).contiguous()
+            self.dur_bias = float(sd[P + dp + "proj.bias"][0])
         self.w = w
 
     @torch.inference_mode()
     def __call__(self, units: torch.Tensor, lang_idx: List[int], spkr_idx: List[int]) -> torch.Tensor:
         """units (B,U) int -> waveform (B,1,U*hop) fp32  (CodeGenerator.forward with dur_prediction=False)."""
+        B, U = units.shape
+        x0 = Seq(B, U, self.cfg.model_in_dim, halo=self.HALO0)
+        self._embed(units, lang_idx, spkr_idx, x0)
+        return self._generate(x0)
+
+    @torch.inference_mode()
+    def resynthesize(self, units: torch.Tensor, lang_idx: List[int], spkr_idx: List[int],
+                     durations: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """CodeGenerator.forward with dur_prediction=True (codehifigan.py:75-101): the duration predictor runs on the unit
+        embeddings, row b's [lang | dict | spkr] frames are repeated by their durations to T_b = sum(dur[b]) frames, and
+        the generator runs on the ragged batch with every row masked to its own length.
+        units (B,U) int -> (wav (B,1,hop*max_b T_b) fp32, zero past hop*T_b in row b; wav_lens (B,) int64 on the host,
+        = hop*T_b; durations (B,U) int32 on the device).  `durations` (B,U) replaces the predicted ones (as
+        VarianceAdaptor.forward(durations=...) does for the T2U)."""
+        x0, lens, tot, dur = self._expand(units, lang_idx, spkr_idx, durations)
+        return self._generate(x0, lens), tot.to(torch.int64) * self.cfg.hop, dur
+
+    def _expand(self, units, lang_idx, spkr_idx, durations=None):
+        """Duration predictor + HardUpsampling of resynthesize() -> (x0 Seq (B, max T_b, model_in_dim) with rows past
+        T_b zero, lens (1+stages, B) int32 on the device, T_b (B,) on the host, durations (B,U) int32)."""
+        if not self.has_dur_predictor:
+            raise NotImplementedError("this vocoder was loaded without duration-predictor weights "
+                                      "(code_generator.dur_predictor.*)")
         lib = _lib.load()
         c, dev, w = self.cfg, self.device, self.w
         B, U = units.shape
         stream = ops._stream()
-        PH = self.HALO0
-        x0 = Seq(B, U, c.model_in_dim, halo=PH)
+        dp = "dur_predictor."
+        xu = Seq(B, U, c.model_in_dim, halo=(c.var_pred_kernel - 1) // 2)
+        self._embed(units, lang_idx, spkr_idx, xu)
+        # VariancePredictor (length_regulator.py:172-218, padding_mask None) on the dict channels of xu, read in place
+        lo = c.lang_embedding_dim
+        xd = Seq(B, U, c.embedding_dim, xu.PH, xu.Tp, buf=xu.buf[:, lo:lo + c.embedding_dim])
+        h1 = ops.gemm(xd, w[dp + "conv1.0.w"], c.var_pred_hidden, w[dp + "conv1.0.b"], taps=c.var_pred_kernel, act=ACT_RELU)
+        h1 = ops.layernorm(h1, w[dp + "ln1.w"], w[dp + "ln1.b"])
+        h2 = ops.gemm(h1, w[dp + "conv2.0.w"], c.var_pred_hidden, w[dp + "conv2.0.b"], taps=c.var_pred_kernel, act=ACT_RELU)
+        h2 = ops.layernorm(h2, w[dp + "ln2.w"], w[dp + "ln2.b"])
+        dur = torch.empty((B, U), dtype=I32, device=dev)
+        check(lib.sb_durations(h2.buf.data_ptr(), h2.Tp, h2.PH, w[dp + "proj.w"].data_ptr(), self.dur_bias,
+                               c.var_pred_hidden, None, B, U, 1.0, dur.data_ptr(), stream), "sb_durations")
+        if durations is not None:
+            if tuple(durations.shape) != (B, U):
+                raise ValueError(f"durations must have shape {(B, U)}, got {tuple(durations.shape)}")
+            dur = durations.to(device=dev, dtype=I32).contiguous()
+        # the one host sync: the expanded length sizes every buffer below (the reference syncs here too, in
+        # repeat_interleave); the per-row totals are summed on the host from the copied durations
+        dur_h = dur.cpu()
+        tot = dur_h.sum(dim=1)
+        if int(dur_h.min()) < 0 or int(tot.min()) < 1:
+            raise ValueError(f"durations must be >= 0 with at least one frame per row (row totals {tot.tolist()})")
+        T = int(tot.max())
+        # row lengths at unit rate and after each upsampling stage, uploaded in one copy
+        scale, scales = 1, [1]
+        for u in c.upsample_rates:
+            scale *= u
+            scales.append(scale)
+        lens = (tot.to(torch.int64)[None, :] * torch.tensor(scales)[:, None]).to(I32).to(dev)
+        x0 = Seq(B, T, c.model_in_dim, halo=self.HALO0, lens=lens[0])
+        # HardUpsampling of [lang | dict | spkr]: rows past each row's total are written as zeros
+        check(lib.sb_upsample_add(xu.buf.data_ptr(), xu.Tp, xu.PH, U, dur.data_ptr(), x0.buf.data_ptr(), x0.Tp, x0.PH, T,
+                                  B, c.model_in_dim, None, None, None, None, 0, 0.0, None, stream), "sb_upsample_add")
+        return x0, lens, tot, dur
+
+    def _embed(self, units: torch.Tensor, lang_idx: List[int], spkr_idx: List[int], x0: Seq) -> None:
+        """x0 data rows = [lang | dict[unit] | spkr] (codehifigan.py:98-100)."""
+        lib = _lib.load()
+        c, dev, w = self.cfg, self.device, self.w
+        B, U = units.shape
+        stream = ops._stream()
         # NOTE: every tensor whose data_ptr() is handed to a kernel must stay referenced until after the launch;
         # a temporary freed earlier can be re-issued by the caching allocator to the next allocation.
         units_i = units.to(I32).contiguous()
@@ -975,6 +1062,15 @@ class VocoderEngine:
                                    w["lang"].data_ptr(), c.lang_embedding_dim, lang_t.data_ptr(), w["spkr"].data_ptr(),
                                    c.spkr_embedding_dim, spkr_t.data_ptr(), x0.buf.data_ptr(), x0.Tp, x0.PH, stream),
               "sb_vocoder_embed")
+
+    def _generate(self, x0: Seq, lens: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Generator.forward (hifigan.py:180-196) on x0 -> (B,1,T*hop) fp32.  lens (1+stages, B) int32: row b's length
+        at unit rate and after each upsampling stage; every conv sees the rows past it as zero padding, and they are 0
+        in the waveform.  None: every row has x0.T frames."""
+        lib = _lib.load()
+        c, dev, w = self.cfg, self.device, self.w
+        B = x0.B
+        stream = ops._stream()
         ch = c.upsample_initial_channel
         act = ops.gemm(x0, w["conv_pre.w"], ch, w["conv_pre.b"], taps=7, act=ACT_LRELU, slope=0.1)  # lrelu fused for ups[0]
         # every buffer below is fully written by a masked sb_gemm except its outermost halo rows (zero="edges")
@@ -985,21 +1081,23 @@ class VocoderEngine:
             # ConvTranspose1d as a 3-tap GEMM producing u*cout values per input frame == u output frames of cout
             T, PHn, Tp = act.T * u, act.PH * u, act.Tp * u
             last_slope = 0.01 if i == nstage - 1 else 0.1  # F.leaky_relu default slope before conv_post (hifigan.py:192)
-            nxt_act = Seq(B, T, cout, PHn, Tp, zero="edges")
+            L = None if lens is None else lens[i + 1]
+            nxt_act = Seq(B, T, cout, PHn, Tp, lens=L, zero="edges")
             fused = self.fused_resblocks and cout in (16, 32) and all(
                 len(dl) == 3 and rk % 2 == 1 and rk <= 11 and (rk - 1) // 2 * max(dl) <= 32
                 for rk, dl in zip(c.resblock_kernel_sizes, c.resblock_dilation_sizes))
-            up_raw = Seq(act.B, act.T, u * cout, act.PH, act.Tp, zero="edges")
-            up_act = None if fused else Seq(act.B, act.T, u * cout, act.PH, act.Tp, zero="edges")
+            # masked at the input rate: row b's T_b input frames give its u*T_b output frames
+            up_raw = Seq(act.B, act.T, u * cout, act.PH, act.Tp, lens=act.lens, zero="edges")
+            up_act = None if fused else Seq(act.B, act.T, u * cout, act.PH, act.Tp, lens=act.lens, zero="edges")
             ops.gemm(act, w[f"ups.{i}.w"], u * cout, w[f"ups.{i}.b"], taps=3, out=up_raw, out2=up_act, out2_slope=0.1)
-            x_raw = Seq(B, T, cout, PHn, Tp, buf=up_raw.buf.view(B * Tp, cout))
+            x_raw = Seq(B, T, cout, PHn, Tp, lens=L, buf=up_raw.buf.view(B * Tp, cout))
             if fused:
                 # narrow stages: each ResBlock is one kernel that keeps its time tile in shared memory (resblock.cu)
                 xs = None
                 for j, (rk, dil) in enumerate(zip(c.resblock_kernel_sizes, c.resblock_dilation_sizes)):
                     rb = i * nk + j
                     lastblock = j == nk - 1
-                    acc = Seq(B, T, cout, PHn, Tp, zero="edges")
+                    acc = Seq(B, T, cout, PHn, Tp, lens=L, zero="edges")
                     names = [f"resblocks.{rb}.convs1.{di}" for di in range(3)], [f"resblocks.{rb}.convs2.{di}" for di in range(3)]
                     ops.hifigan_resblock(x_raw, [w[n + ".w"] for n in names[0]], [w[n + ".b"] for n in names[0]],
                                          [w[n + ".w"] for n in names[1]], [w[n + ".b"] for n in names[1]], rk, list(dil),
@@ -1008,7 +1106,7 @@ class VocoderEngine:
                     xs = acc
                 act = nxt_act
                 continue
-            x_act = Seq(B, T, cout, PHn, Tp, buf=up_act.buf.view(B * Tp, cout))
+            x_act = Seq(B, T, cout, PHn, Tp, lens=L, buf=up_act.buf.view(B * Tp, cout))
             xs = None
             for j, (rk, dil) in enumerate(zip(c.resblock_kernel_sizes, c.resblock_dilation_sizes)):
                 rb = i * nk + j
@@ -1018,7 +1116,8 @@ class VocoderEngine:
                                   dil=d, act=ACT_LRELU, slope=0.1)
                     lastpair = di == len(dil) - 1
                     if not lastpair:
-                        n_raw, n_act = Seq(B, T, cout, PHn, Tp, zero="edges"), Seq(B, T, cout, PHn, Tp, zero="edges")
+                        n_raw = Seq(B, T, cout, PHn, Tp, lens=L, zero="edges")
+                        n_act = Seq(B, T, cout, PHn, Tp, lens=L, zero="edges")
                         ops.gemm(t1, w[f"resblocks.{rb}.convs2.{di}.w"], cout, w[f"resblocks.{rb}.convs2.{di}.b"], taps=rk,
                                  res1=y_raw, out=n_raw, out2=n_act, out2_slope=0.1)
                         y_raw, y_act = n_raw, n_act
@@ -1026,7 +1125,7 @@ class VocoderEngine:
                         # xs (+)= resblock output; the last resblock also applies the 1/num_kernels mean and the
                         # leaky-relu that feeds the next stage (hifigan.py:186-192)
                         lastblock = j == nk - 1
-                        acc = Seq(B, T, cout, PHn, Tp, zero="edges")
+                        acc = Seq(B, T, cout, PHn, Tp, lens=L, zero="edges")
                         ops.gemm(t1, w[f"resblocks.{rb}.convs2.{di}.w"], cout, w[f"resblocks.{rb}.convs2.{di}.b"], taps=rk,
                                  res1=y_raw, res2=xs, gamma=(1.0 / nk) if lastblock else 1.0, out=acc,
                                  out2=nxt_act if lastblock else None, out2_slope=last_slope)
@@ -1034,6 +1133,7 @@ class VocoderEngine:
             act = nxt_act
         Tw = act.T
         wav = torch.empty((B, Tw), dtype=torch.float32, device=dev)
-        check(lib.sb_conv_post_tanh(act.buf.data_ptr(), act.Tp, act.PH, Tw, act.C, B, w["conv_post.w"].data_ptr(),
-                                    self.conv_post_bias, 7, wav.data_ptr(), wav.stride(0), stream), "sb_conv_post_tanh")
+        check(lib.sb_conv_post_tanh(act.buf.data_ptr(), act.Tp, act.PH, Tw, ops._p(act.lens), act.C, B,
+                                    w["conv_post.w"].data_ptr(), self.conv_post_bias, 7, wav.data_ptr(), wav.stride(0),
+                                    stream), "sb_conv_post_tanh")
         return wav.view(B, 1, Tw)

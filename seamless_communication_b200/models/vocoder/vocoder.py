@@ -15,6 +15,7 @@ class Vocoder:
     def __init__(self, engine: VocoderEngine, lang_spkr_idx_map: Dict[str, Any]):
         self.code_generator = engine
         self.lang_spkr_idx_map = lang_spkr_idx_map
+        self.last_wav_lens: Optional[Tensor] = None  # (N,) int64 samples per row of the last dur_prediction=True call
 
     def eval(self):
         return self
@@ -22,7 +23,13 @@ class Vocoder:
     def forward(self, units: Tensor, lang_list: Union[List[str], str], spkr_list: Union[Optional[List[int]], int] = None,
                 dur_prediction: bool = True) -> Tensor:
         """Same argument conventions as the reference's Vocoder.forward (models/vocoder/vocoder.py:25-49): a single
-        language / speaker applies to the whole batch, speaker -1 (or None) selects the language's first speaker."""
+        language / speaker applies to the whole batch, speaker -1 (or None) selects the language's first speaker.
+
+        dur_prediction=True (the reference's default, for deduplicated units) repeats each unit by the duration the
+        vocoder's own predictor gives it.  Rows may then differ in length: the output is (N, 1, hop * max_b T_b), row b
+        is zero past its own hop * T_b samples, and `last_wav_lens` holds those per-row sample counts.  It needs a
+        vocoder loaded with its duration predictor (code_generator.dur_predictor.*); without one it raises
+        NotImplementedError."""
         if units.dim() == 1:
             units = units[None]
         n = units.size(0)
@@ -35,8 +42,11 @@ class Vocoder:
         lang_ids = [table["multilingual"][name] for name in langs]
         spkr_ids = [table["multispkr"][name][0] if s == -1 else s for name, s in zip(langs, spkrs)]
         if dur_prediction:
-            # only the AR-T2U (v1) models need the vocoder's own duration predictor (translator.py:381-394)
-            raise NotImplementedError("vocoder duration prediction belongs to the v1 AR T2U path (SURVEY 8f.4)")
+            if not getattr(self.code_generator, "has_dur_predictor", False):
+                raise NotImplementedError("dur_prediction=True needs a vocoder loaded with its duration predictor "
+                                          "(code_generator.dur_predictor.*)")
+            wav, self.last_wav_lens, _ = self.code_generator.resynthesize(units.reshape(n, -1), lang_ids, spkr_ids)
+            return wav
         return self.code_generator(units.reshape(n, -1), lang_ids, spkr_ids)
 
     __call__ = forward

@@ -115,7 +115,8 @@ def gemm_raw(a: torch.Tensor, w: torch.Tensor, n: int, bias=None, *, act=ACT_NON
 
 def hifigan_resblock(x: Seq, w1, b1, w2, b2, k: int, dil, *, res2: Optional[Seq] = None, gamma=1.0, out: Seq,
                      out2: Optional[Seq] = None, out2_slope=0.0, slope=0.1) -> Seq:
-    """One fused HiFi-GAN ResBlock (hifigan.py:33-121) on a 16- or 32-channel Seq: out = (resblock(x) + res2) * gamma."""
+    """One fused HiFi-GAN ResBlock (hifigan.py:33-121) on a 16- or 32-channel Seq: out = (resblock(x) + res2) * gamma.
+    With x.lens, rows past each sequence's length are zero padding and are written as 0."""
     lib = _lib.load()
     assert len(dil) == 3 and len(w1) == len(w2) == len(b1) == len(b2) == 3
     assert x.Tp == x.T + 2 * x.PH and x.buf.stride(0) == x.C
@@ -128,6 +129,7 @@ def hifigan_resblock(x: Seq, w1, b1, w2, b2, k: int, dil, *, res2: Optional[Seq]
     d.channels, d.kernel_size = x.C, k
     d.batch, d.T, d.rows_per_seq, d.halo = x.B, x.T, x.Tp, x.PH
     d.slope, d.gamma, d.out2_slope = slope, gamma, out2_slope
+    d.lens = _p(x.lens)
     check(lib.sb_hifigan_resblock(C.byref(d), _stream()), "sb_hifigan_resblock")
     return out
 

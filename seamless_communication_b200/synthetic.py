@@ -169,10 +169,15 @@ def make_unity_state_dict(cfg: UnitYConfig, seed: int = 0, logit_scale: float = 
     return I.sd
 
 
-def make_vocoder_state_dict(cfg: VocoderConfig, seed: int = 1) -> Dict[str, torch.Tensor]:
+def make_vocoder_state_dict(cfg: VocoderConfig, seed: int = 1, dur_predictor: bool = False, dur_gain: float = 0.3,
+                            dur_bias: float = 1.0) -> Dict[str, torch.Tensor]:
     """Random-init Code-HiFiGAN parameters, weight-norm parametrised (weight_g/weight_v) exactly as the
     reference checkpoint stores them (models/vocoder/hifigan.py:44-176; loader.py:24-36).
-    weight_g is drawn around ||v|| (PyTorch's default is exactly ||v||) so folding g*v/||v|| is exercised."""
+    weight_g is drawn around ||v|| (PyTorch's default is exactly ||v||) so folding g*v/||v|| is exercised.
+
+    dur_predictor=True adds the duration predictor (codehifigan.py:45-47, a VariancePredictor), drawn from its own
+    generator so that every other tensor is the same as without it.  With the default dur_gain / dur_bias the predicted
+    log-durations l spread about 1.0 +- 0.4, so round(exp(l) - 1) runs from clamped 1s to 5 or more (mean about 2)."""
     I = _Init(seed)
     P = "code_generator"
 
@@ -200,6 +205,16 @@ def make_vocoder_state_dict(cfg: VocoderConfig, seed: int = 1) -> Dict[str, torc
                 wn_conv(f"resblocks.{rb}.convs1.{d}", cout, cout, rk, gain=1.2)
                 wn_conv(f"resblocks.{rb}.convs2.{d}", cout, cout, rk, gain=0.6)
     wn_conv("conv_post", 1, ch // (2 ** len(cfg.upsample_rates)), 7, gain=0.25)
+    if dur_predictor:
+        D = _Init(seed + 1000)
+        p = f"{P}.dur_predictor"
+        D.conv(f"{p}.conv1.0", cfg.var_pred_hidden, cfg.embedding_dim, cfg.var_pred_kernel)
+        D.ln(f"{p}.ln1", cfg.var_pred_hidden)
+        D.conv(f"{p}.conv2.0", cfg.var_pred_hidden, cfg.var_pred_hidden, cfg.var_pred_kernel)
+        D.ln(f"{p}.ln2", cfg.var_pred_hidden)
+        D.linear(f"{p}.proj", 1, cfg.var_pred_hidden, gain=dur_gain)
+        D.sd[f"{p}.proj.bias"] = _round_fp16(torch.tensor([dur_bias]))
+        I.sd.update(D.sd)
     return I.sd
 
 
