@@ -141,6 +141,17 @@ int sb_attention(const void* q, int64_t q_ld, const void* k, int64_t k_ld, const
                  int64_t out_ld, int32_t batch, int32_t heads, int32_t sq, int32_t sk, int32_t q_rows, int32_t q_halo,
                  int32_t kv_rows, int32_t kv_halo, const int32_t* kv_lens, int32_t causal, const void* rel_k,
                  int32_t rel_left, int32_t rel_right, sb_stream_t stream);
+/* sb_attention_relpos - Transformer-XL relative-position self-attention of w2v-BERT v1 (RelativePositionSDPA, mirrored
+ * fairseq2.cpp:605-696), same layouts and key mask as sb_attention, sq = sk = s, no causal mode:
+ *   scores[i][j] = ((q_i + u) . k_j + (q_i + v) . R[s-1+j-i]) / 8
+ * r: fp16 [2s-1][r_ld], head h in columns h*64..h*64+63 (R = r_proj(pos table rows n_ctx-s .. n_ctx+s-2)); u, v: fp32
+ * [heads][64] or NULL (= 0); q + u and q + v are summed in fp32 and rounded once to fp16.  SB_ENOSUP for s > 4096 (the
+ * relative position table covers distances up to 4095), before anything is launched.
+ * ---------------------------------------------------------------------------------------------------------------- */
+int sb_attention_relpos(const void* q, int64_t q_ld, const void* k, int64_t k_ld, const void* v, int64_t v_ld, void* out,
+                        int64_t out_ld, int32_t batch, int32_t heads, int32_t s, int32_t q_rows, int32_t q_halo,
+                        int32_t kv_rows, int32_t kv_halo, const int32_t* kv_lens, const void* r, int64_t r_ld,
+                        const float* u, const float* v_bias, sb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * sb_dwconv_ln_silu - Conformer conv module middle: causal depthwise Conv1d(k) -> LayerNorm(C) -> SiLU.
@@ -149,6 +160,10 @@ int sb_attention(const void* q, int64_t q_ld, const void* k, int64_t k_ld, const
  * ---------------------------------------------------------------------------------------------------------------- */
 int sb_dwconv_ln_silu(const void* x, void* y, const void* w, const float* ln_w, const float* ln_b, int32_t batch,
                       int32_t T, int32_t C, int32_t k, sb_stream_t stream);
+/* sb_dwconv_bias_silu - the w2v-BERT v1 form: depthwise Conv1d(k = 31, pad 15 on both sides) -> + bias[c] -> SiLU, with
+ * BatchNorm's scale already folded into w (fairseq2.cpp:698-731).  Frames outside [0, T) read as zero.  C % 64 == 0, C <= 1024. */
+int sb_dwconv_bias_silu(const void* x, void* y, const void* w, const float* bias, int32_t batch, int32_t T, int32_t C,
+                        int32_t k, sb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Text decoder step pieces (KV cache with beam-ancestor indirection instead of the reference's per-step

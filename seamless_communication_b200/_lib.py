@@ -97,7 +97,10 @@ PROTOTYPES = {
     "sb_layernorm": [c_p, c_p, c_p, c_p, c_p, c_p, i32, i32, i32, i32, i32, i32, i32, c_p, i32, c_p],
     "sb_attention": [c_p, i64, c_p, i64, c_p, i64, c_p, i64, i32, i32, i32, i32, i32, i32, i32, i32, c_p, i32, c_p, i32,
                      i32, c_p],
+    "sb_attention_relpos": [c_p, i64, c_p, i64, c_p, i64, c_p, i64, i32, i32, i32, i32, i32, i32, i32, c_p, c_p, i64, c_p,
+                            c_p, c_p],
     "sb_dwconv_ln_silu": [c_p, c_p, c_p, c_p, c_p, i32, i32, i32, i32, c_p],
+    "sb_dwconv_bias_silu": [c_p, c_p, c_p, c_p, i32, i32, i32, i32, c_p],
     "sb_embed_step": [c_p, i32, c_p, c_p, c_p, f32, c_p, i32, i32, c_p],
     "sb_step_advance": [c_p, c_p],
     "sb_store_step": [c_p, c_p, c_p, i64, c_p],

@@ -6,10 +6,13 @@ registries (reference: src/seamless_communication/models/unity/builder.py:165-19
 models/conformer_shaw/builder.py:55-68, models/vocoder/builder.py:42-64
 `_base_vocoder`).  Only the fields the hot path reads are kept.
 
-Two named architectures exist:
+Named architectures:
   * ``base_v2``  - seamlessM4T_v2_large (the headline configuration);
-  * ``tiny_v2``  - same topology, small dims, used by the parity tests so the
-    CPU oracle finishes in seconds.
+  * ``tiny_v2`` / ``small_v2`` - same topology, small dims / few layers, used by
+    the parity tests so the CPU oracle finishes in seconds;
+  * ``base``     - seamlessM4T_large (builder.py:109-134, w2v-BERT v1 speech
+    encoder, same 600m / dense_1b dims), with ``tiny_v1`` / ``small_v1`` test
+    copies.  Only speech-to-text runs on them: they carry no T2U.
 """
 from __future__ import annotations
 
@@ -64,6 +67,9 @@ class UnitYConfig:
     dw_kernel: int = 31
     shaw_left: int = 64
     shaw_right: int = 8
+    # "v2": Shaw relative attention, causal depthwise conv + LayerNorm (w2v-BERT 2.0);
+    # "v1": Transformer-XL relative attention, symmetric depthwise conv + BatchNorm (w2v-BERT v1, seamlessM4T_large)
+    encoder_variant: str = "v2"
     # --- adaptor (builder.py:188-192) ---
     adaptor_kernel: int = 8
     adaptor_stride: int = 8
@@ -177,6 +183,23 @@ def small_v2() -> UnitYConfig:
     )
 
 
+def base() -> UnitYConfig:
+    """seamlessM4T_large: the base_v2 dims with the w2v-BERT v1 encoder; speech-to-text only here (no T2U)."""
+    return UnitYConfig(name="base", encoder_variant="v1")
+
+
+def tiny_v1() -> UnitYConfig:
+    c = tiny_v2()
+    c.name, c.encoder_variant = "tiny_v1", "v1"
+    return c
+
+
+def small_v1() -> UnitYConfig:
+    c = small_v2()
+    c.name, c.encoder_variant = "small_v1", "v1"
+    return c
+
+
 def base_vocoder() -> VocoderConfig:
     return VocoderConfig()
 
@@ -193,10 +216,12 @@ def tiny_vocoder() -> VocoderConfig:
     )
 
 
-UNITY_ARCHS = {"base_v2": base_v2, "tiny_v2": tiny_v2, "small_v2": small_v2}
+UNITY_ARCHS = {"base_v2": base_v2, "tiny_v2": tiny_v2, "small_v2": small_v2, "base": base, "tiny_v1": tiny_v1,
+               "small_v1": small_v1}
 VOCODER_ARCHS = {"base": base_vocoder, "tiny": tiny_vocoder}
 
 # asset-card names the reference resolves through fairseq2's asset store
 # (cards/seamlessM4T_v2_large.yaml: model_arch base_v2; cards/vocoder_v2.yaml: base)
-MODEL_CARDS = {"seamlessM4T_v2_large": "base_v2", "seamlessM4T_v2_tiny": "tiny_v2", "seamlessM4T_v2_small": "small_v2"}
+MODEL_CARDS = {"seamlessM4T_v2_large": "base_v2", "seamlessM4T_v2_tiny": "tiny_v2", "seamlessM4T_v2_small": "small_v2",
+               "seamlessM4T_large": "base"}
 VOCODER_CARDS = {"vocoder_v2": "base", "vocoder_v2_tiny": "tiny"}

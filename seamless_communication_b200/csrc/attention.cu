@@ -5,7 +5,14 @@
 // Shaw relative-position bias (models/conformer_shaw/builder.py:127-146): instead of the reference's (S,S,64) gather
 // + einsum, each warp computes QR = q . rel_k^T once (16 x 73, a tiny GEMM) and the score tile adds
 // QR[i, clamp(j-i,-L,R)+L] by a shared-memory lookup.
+// Transformer-XL relative attention of w2v-BERT v1 (RelativePositionSDPA; mirrored ggml/examples/unity/fairseq2.cpp:605-696):
+// scores[i][j] = ((q_i + u).k_j + (q_i + v).R[S-1+j-i]) / 8, R = r_proj(pos table) of shape (2S-1, H*64).  The (S, 2S-1)
+// positional scores are never materialised: for each 64 x 64 (query, key) tile the 127 R rows it touches are staged in shared
+// memory (a 128-row window), each warp multiplies its 16 rows of q + v against the 80 rows its queries reach (16 x 80, five
+// m16n8k16 column pairs) and the score tile adds them by diagonal lookup: row il, key jl reads column jl - il + 15.
 #include "common.cuh"
+
+#include <type_traits>
 
 namespace sb {
 
@@ -13,6 +20,8 @@ constexpr int HD = 64;          // head dim
 constexpr int AQ = 64, AK = 64; // query / key block
 constexpr int LDS = HD + 8;     // padded smem row (halves): conflict-free ldmatrix
 constexpr int REL_MAX = 80;     // rel table rows padded to a multiple of 16
+constexpr int XL_ROWS = 128;    // R window per (query tile, key tile): rows S-1+k0-q0-63 .. +127 (the last one unused)
+constexpr int XL_MAX_S = 4096;  // fairseq2's relative position table covers distances up to n_ctx - 1 = 4095
 
 __device__ __forceinline__ void ldsm_x4(uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3, const void* p) {
   uint32_t a = (uint32_t)__cvta_generic_to_shared(p);
@@ -43,29 +52,61 @@ struct AttnArgs {
   const elem_t* rel_k;
   int rel_left, rel_right;
 };
+// Transformer-XL mode: R fp16 [2*sq-1][r_ld] (head h at columns h*64..), u / v fp32 [heads][64] (NULL = 0)
+struct XlAttnArgs : AttnArgs {
+  const elem_t* r;
+  long long r_ld;
+  const float *bias_u, *bias_v;
+};
 
-__global__ void __launch_bounds__(128) attention_kernel(const AttnArgs p) {
+// XL = false: plain or Shaw attention (sb_attention); XL = true: Transformer-XL relative attention (sb_attention_relpos)
+template <bool XL>
+__global__ void __launch_bounds__(128) attention_kernel(const std::conditional_t<XL, XlAttnArgs, AttnArgs> p) {
   extern __shared__ __align__(16) uint8_t smem_attn[];
-  elem_t* sQ = reinterpret_cast<elem_t*>(smem_attn);  // [AQ][LDS]
+  elem_t* sQ = reinterpret_cast<elem_t*>(smem_attn);  // [AQ][LDS]   (XL: q + u)
   elem_t* sK = sQ + AQ * LDS;                         // [AK][LDS]
   elem_t* sV = sK + AK * LDS;                         // [AK][LDS]
-  elem_t* sR = sV + AK * LDS;                         // [REL_MAX][LDS]   (Shaw only)
-  float* sQR = reinterpret_cast<float*>(sR + REL_MAX * LDS);  // [4 warps][16][REL_MAX+1]
+  elem_t* sR = sV + AK * LDS;                         // [REL_MAX][LDS]   (Shaw) / [XL_ROWS][LDS] (XL: R window)
+  float* sQR = reinterpret_cast<float*>(sR + (XL ? XL_ROWS : REL_MAX) * LDS);  // [4 warps][16][REL_MAX+1]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, tq = lane & 3;
   const int q0 = blockIdx.x * AQ;
   const int h = blockIdx.y, b = blockIdx.z;
   const int kv_len = p.kv_lens ? min(p.kv_lens[b], p.sk) : p.sk;
-  const bool shaw = p.rel_k != nullptr;
+  const bool shaw = !XL && p.rel_k != nullptr;
   const int nrel = p.rel_left + p.rel_right + 1;
 
   // ---- stage Q tile (and the rel table) ----
-  for (int i = threadIdx.x; i < AQ * (HD / 8); i += blockDim.x) {
-    int r = i / (HD / 8), c = (i % (HD / 8)) * 8;
-    uint4 u = make_uint4(0, 0, 0, 0);
-    if (q0 + r < p.sq) u = *reinterpret_cast<const uint4*>(p.q + ((long long)b * p.q_rows + p.q_halo + q0 + r) * p.q_ld + h * HD + c);
-    *reinterpret_cast<uint4*>(sQ + r * LDS + c) = u;
+  if constexpr (XL) {
+    // sQ = q + u, sQv = q + v: summed in fp32, rounded once to fp16 (with u == NULL, sQ is q bit for bit)
+    elem_t* sQv = reinterpret_cast<elem_t*>(sQR + 4 * 16 * (REL_MAX + 1));  // [AQ][LDS]
+    for (int i = threadIdx.x; i < AQ * (HD / 8); i += blockDim.x) {
+      int r = i / (HD / 8), c = (i % (HD / 8)) * 8;
+      uint4 qu = make_uint4(0, 0, 0, 0), qv = make_uint4(0, 0, 0, 0);
+      if (q0 + r < p.sq) {
+        const uint4 raw = *reinterpret_cast<const uint4*>(p.q + ((long long)b * p.q_rows + p.q_halo + q0 + r) * p.q_ld + h * HD + c);
+        const __half2* hq = reinterpret_cast<const __half2*>(&raw);
+        __half2* hu = reinterpret_cast<__half2*>(&qu);
+        __half2* hv = reinterpret_cast<__half2*>(&qv);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float2 f = __half22float2(hq[e]);
+          const int o = h * HD + c + 2 * e;
+          hu[e] = p.bias_u ? __floats2half2_rn(f.x + p.bias_u[o], f.y + p.bias_u[o + 1]) : hq[e];
+          hv[e] = p.bias_v ? __floats2half2_rn(f.x + p.bias_v[o], f.y + p.bias_v[o + 1]) : hq[e];
+        }
+      }
+      *reinterpret_cast<uint4*>(sQ + r * LDS + c) = qu;
+      *reinterpret_cast<uint4*>(sQv + r * LDS + c) = qv;
+    }
+  } else {
+    for (int i = threadIdx.x; i < AQ * (HD / 8); i += blockDim.x) {
+      int r = i / (HD / 8), c = (i % (HD / 8)) * 8;
+      uint4 u = make_uint4(0, 0, 0, 0);
+      if (q0 + r < p.sq) u = *reinterpret_cast<const uint4*>(p.q + ((long long)b * p.q_rows + p.q_halo + q0 + r) * p.q_ld + h * HD + c);
+      *reinterpret_cast<uint4*>(sQ + r * LDS + c) = u;
+    }
   }
   if (shaw) {
     for (int i = threadIdx.x; i < REL_MAX * (HD / 8); i += blockDim.x) {
@@ -83,6 +124,15 @@ __global__ void __launch_bounds__(128) attention_kernel(const AttnArgs p) {
   for (int ks = 0; ks < 4; ++ks) {
     const elem_t* ptr = sQ + (warp * 16 + (lane & 7) + 8 * ((lane >> 3) & 1)) * LDS + ks * 16 + 8 * (lane >> 4);
     ldsm_x4(qa[ks][0], qa[ks][1], qa[ks][2], qa[ks][3], ptr);
+  }
+  uint32_t qva[XL ? 4 : 1][4];  // XL: (q + v) fragments
+  if constexpr (XL) {
+    const elem_t* sQv = reinterpret_cast<const elem_t*>(sQR + 4 * 16 * (REL_MAX + 1));
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+      const elem_t* ptr = sQv + (warp * 16 + (lane & 7) + 8 * ((lane >> 3) & 1)) * LDS + ks * 16 + 8 * (lane >> 4);
+      ldsm_x4(qva[ks][0], qva[ks][1], qva[ks][2], qva[ks][3], ptr);
+    }
   }
   float* qr = sQR + warp * 16 * (REL_MAX + 1);
   if (shaw) {
@@ -133,7 +183,44 @@ __global__ void __launch_bounds__(128) attention_kernel(const AttnArgs p) {
       *reinterpret_cast<uint4*>(sK + r * LDS + c) = uk;
       *reinterpret_cast<uint4*>(sV + r * LDS + c) = uv;
     }
+    if constexpr (XL) {
+      // R rows S-1+j-i for j in [k0, k0+64), i in [q0, q0+64): window base S-1+k0-q0-63; rows outside [0, 2S-1) read as 0
+      const int rbase = p.sq - 1 + k0 - q0 - (AQ - 1);
+      for (int i = threadIdx.x; i < XL_ROWS * (HD / 8); i += blockDim.x) {
+        int r = i / (HD / 8), c = (i % (HD / 8)) * 8;
+        const int row = rbase + r;
+        uint4 u = make_uint4(0, 0, 0, 0);
+        if (row >= 0 && row < 2 * p.sq - 1) u = *reinterpret_cast<const uint4*>(p.r + (long long)row * p.r_ld + h * HD + c);
+        *reinterpret_cast<uint4*>(sR + r * LDS + c) = u;
+      }
+    }
     __syncthreads();
+    if constexpr (XL) {
+      // QR[il][n] = (q + v)_{q0+16w+il} . R[rbase + 48 - 16w + n], n < 80: column jl - il + 15 holds key k0 + jl
+      const elem_t* sRw = sR + (AQ - 16 - 16 * warp) * LDS;
+#pragma unroll
+      for (int nt2 = 0; nt2 < REL_MAX / 16; ++nt2) {
+        float c0[4] = {0, 0, 0, 0}, c1[4] = {0, 0, 0, 0};
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) {
+          uint32_t b0, b1, b2, b3;
+          const elem_t* ptr = sRw + (nt2 * 16 + (lane & 7) + 8 * (lane >> 4)) * LDS + ks * 16 + 8 * ((lane >> 3) & 1);
+          ldsm_x4(b0, b1, b2, b3, ptr);
+          mma16816(c0, qva[ks], b0, b1);
+          mma16816(c1, qva[ks], b2, b3);
+        }
+        const int col = nt2 * 16 + 2 * tq;
+        qr[g * (REL_MAX + 1) + col] = c0[0];
+        qr[g * (REL_MAX + 1) + col + 1] = c0[1];
+        qr[(g + 8) * (REL_MAX + 1) + col] = c0[2];
+        qr[(g + 8) * (REL_MAX + 1) + col + 1] = c0[3];
+        qr[g * (REL_MAX + 1) + col + 8] = c1[0];
+        qr[g * (REL_MAX + 1) + col + 9] = c1[1];
+        qr[(g + 8) * (REL_MAX + 1) + col + 8] = c1[2];
+        qr[(g + 8) * (REL_MAX + 1) + col + 9] = c1[3];
+      }
+      __syncwarp();
+    }
 
     // S = Q K^T  (16 x 64 per warp)
     float s[8][4];
@@ -160,7 +247,9 @@ __global__ void __launch_bounds__(128) attention_kernel(const AttnArgs p) {
         const int i = irow[rr];
         const int j = k0 + nt * 8 + 2 * tq + (e & 1);
         float val = s[nt][e];
-        if (shaw) {
+        if constexpr (XL) {
+          val += qr[(g + 8 * rr) * (REL_MAX + 1) + nt * 8 + 2 * tq + (e & 1) - (g + 8 * rr) + 15];
+        } else if (shaw) {
           int d = j - i;
           d = d < -p.rel_left ? -p.rel_left : (d > p.rel_right ? p.rel_right : d);
           val += qr[(g + 8 * rr) * (REL_MAX + 1) + d + p.rel_left];
@@ -533,11 +622,39 @@ extern "C" int sb_attention(const void* q, int64_t q_ld, const void* k, int64_t 
   if (rel_k) smem += (size_t)REL_MAX * LDS * sizeof(elem_t) + 4 * 16 * (REL_MAX + 1) * sizeof(float);
   static bool configured = false;
   if (!configured) {
-    SB_CUDA_OK(cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+    SB_CUDA_OK(cudaFuncSetAttribute(attention_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
     configured = true;
   }
   dim3 grid((sq + AQ - 1) / AQ, heads, batch);
-  attention_kernel<<<grid, 128, smem, (cudaStream_t)stream>>>(a);
+  attention_kernel<false><<<grid, 128, smem, (cudaStream_t)stream>>>(a);
+  SB_LAUNCH_OK();
+  return SB_OK;
+}
+
+extern "C" int sb_attention_relpos(const void* q, int64_t q_ld, const void* k, int64_t k_ld, const void* v, int64_t v_ld,
+                                   void* out, int64_t out_ld, int32_t batch, int32_t heads, int32_t s, int32_t q_rows,
+                                   int32_t q_halo, int32_t kv_rows, int32_t kv_halo, const int32_t* kv_lens, const void* r,
+                                   int64_t r_ld, const float* bias_u, const float* bias_v, sb_stream_t stream) {
+  using namespace sb;
+  SB_REQUIRE(q && k && v && out && r && batch > 0 && heads > 0 && s > 0, SB_EINVAL, "sb_attention_relpos: bad args");
+  SB_REQUIRE(s <= XL_MAX_S, SB_ENOSUP, "sb_attention_relpos: sequence length %d exceeds %d", s, XL_MAX_S);
+  SB_REQUIRE((q_ld % 8) == 0 && (k_ld % 8) == 0 && (v_ld % 8) == 0 && (r_ld % 8) == 0 && (out_ld % 2) == 0, SB_ENOSUP,
+             "sb_attention_relpos: row strides must be multiples of 8 elements");
+  XlAttnArgs a = {};
+  a.q = (const elem_t*)q; a.k = (const elem_t*)k; a.v = (const elem_t*)v; a.out = (elem_t*)out;
+  a.q_ld = q_ld; a.k_ld = k_ld; a.v_ld = v_ld; a.out_ld = out_ld;
+  a.batch = batch; a.heads = heads; a.sq = s; a.sk = s; a.q_rows = q_rows; a.q_halo = q_halo;
+  a.kv_rows = kv_rows; a.kv_halo = kv_halo; a.kv_lens = kv_lens;
+  a.r = (const elem_t*)r; a.r_ld = r_ld; a.bias_u = bias_u; a.bias_v = bias_v;
+  // Q, K, V, the 128-row R window, the per-warp 16 x 81 fp32 QR tiles and the (q + v) tile: 77 KB
+  const size_t smem = (size_t)(AQ + 2 * AK + XL_ROWS + AQ) * LDS * sizeof(elem_t) + 4 * 16 * (REL_MAX + 1) * sizeof(float);
+  static bool configured = false;
+  if (!configured) {
+    SB_CUDA_OK(cudaFuncSetAttribute(attention_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    configured = true;
+  }
+  dim3 grid((s + AQ - 1) / AQ, heads, batch);
+  attention_kernel<true><<<grid, 128, smem, (cudaStream_t)stream>>>(a);
   SB_LAUNCH_OK();
   return SB_OK;
 }

@@ -1,5 +1,8 @@
 // sb_dwconv_ln_silu: Conformer convolution module core for w2v-BERT 2.0 (conformer_shaw/builder.py:148-156):
 //   causal depthwise Conv1d(kernel k, left pad k-1, no bias) -> LayerNorm(C) -> SiLU,   x,y: (B,T,C) fp16.
+// sb_dwconv_bias_silu: the same core for w2v-BERT v1 (ConvModule_forward, ggml/examples/unity/fairseq2.cpp:698-731):
+//   depthwise Conv1d(k = 31, pad 15 on both sides) -> BatchNorm (eval statistics) -> SiLU, with the BatchNorm scale folded
+//   into the depthwise weights by the host, so that only a per-channel bias remains.
 // (the pointwise convs and the GLU live in the sb_gemm epilogues around it.)
 // One CTA = TT output frames x all C channels.  The (TT+k-1) x C input window is staged once in shared memory
 // (each input element is reused k times from smem instead of HBM/L2), conv results stay in smem as fp32 for the
@@ -161,6 +164,9 @@ __device__ __forceinline__ void dw_cp_async16(void* smem_dst, const void* gsrc) 
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
 }
 
+// V1 = true (sb_dwconv_bias_silu): window t0-15 .. t0+46 (symmetric padding), no LayerNorm; ln_w then holds the per-channel
+// bias that follows the folded BatchNorm and ln_b is unused.
+template <bool V1>
 __global__ void __launch_bounds__(512) dwconv31_tile_kernel(const elem_t* __restrict__ x, elem_t* __restrict__ y,
                                                              const elem_t* __restrict__ w, const float* __restrict__ ln_w,
                                                              const float* __restrict__ ln_b, int T, int C) {
@@ -175,7 +181,7 @@ __global__ void __launch_bounds__(512) dwconv31_tile_kernel(const elem_t* __rest
   const int vec_per_row = C / 8;
   for (int i = threadIdx.x; i < DW2_ROWS * vec_per_row; i += blockDim.x) {
     const int r = i / vec_per_row, c = (i - r * vec_per_row) * 8;
-    const int t = t0 - (DW2_K - 1) + r;
+    const int t = t0 - (V1 ? DW2_K / 2 : DW2_K - 1) + r;
     elem_t* dst = sx + (size_t)r * C + c;
     if (t >= 0 && t < T) dw_cp_async16(dst, xb + (long long)t * C + c);
     else *reinterpret_cast<uint4*>(dst) = make_uint4(0, 0, 0, 0);
@@ -199,7 +205,8 @@ __global__ void __launch_bounds__(512) dwconv31_tile_kernel(const elem_t* __rest
 #pragma unroll
     for (int j = 0; j < DW2_K; ++j) { wa[j] = h[j]; wb[j] = h[DW2_K + j]; }
   }
-  const float2 g = *reinterpret_cast<const float2*>(ln_w + c), be = *reinterpret_cast<const float2*>(ln_b + c);
+  const float2 g = *reinterpret_cast<const float2*>(ln_w + c);
+  const float2 be = V1 ? make_float2(0.f, 0.f) : *reinterpret_cast<const float2*>(ln_b + c);
 #pragma unroll 1
   for (int pass = 0; pass < DW2_TT / DW2_PASS; ++pass) {
     const int f0 = pass * DW2_PASS;  // first output frame of the pass inside the tile; it reads rows f0 .. f0 + 45
@@ -216,6 +223,19 @@ __global__ void __launch_bounds__(512) dwconv31_tile_kernel(const elem_t* __rest
           acc[t].y += wb[r - t] * xv.y;
         }
       }
+    }
+    if constexpr (V1) {
+#pragma unroll
+      for (int t = 0; t < DW2_PASS; ++t) {
+        const int tt = t0 + f0 + t;
+        if (tt < T) {
+          float a0 = acc[t].x + g.x, a1 = acc[t].y + g.y;
+          a0 = a0 / (1.f + __expf(-a0));
+          a1 = a1 / (1.f + __expf(-a1));
+          *reinterpret_cast<__half2*>(y + ((long long)b * T + tt) * C + c) = __floats2half2_rn(a0, a1);
+        }
+      }
+      continue;
     }
     // LayerNorm statistics of the 16 frames over all channels
 #pragma unroll
@@ -267,10 +287,10 @@ extern "C" int sb_dwconv_ln_silu(const void* x, void* y, const void* w, const fl
     if (tile_ok && smem2 <= 220 * 1024) {
       static size_t configured2 = 0;
       if (smem2 > configured2) {
-        SB_CUDA_OK(cudaFuncSetAttribute(dwconv31_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
+        SB_CUDA_OK(cudaFuncSetAttribute(dwconv31_tile_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
         configured2 = smem2;
       }
-      dwconv31_tile_kernel<<<dim3((T + DW2_TT - 1) / DW2_TT, batch), threads, smem2, (cudaStream_t)stream>>>(
+      dwconv31_tile_kernel<false><<<dim3((T + DW2_TT - 1) / DW2_TT, batch), threads, smem2, (cudaStream_t)stream>>>(
           (const elem_t*)x, (elem_t*)y, (const elem_t*)w, ln_w, ln_b, T, C);
       SB_LAUNCH_OK();
       return SB_OK;
@@ -300,6 +320,25 @@ extern "C" int sb_dwconv_ln_silu(const void* x, void* y, const void* w, const fl
   }
   dwconv_ln_silu_kernel<<<grid, DW_THREADS, smem, (cudaStream_t)stream>>>((const elem_t*)x, (elem_t*)y, (const elem_t*)w, ln_w,
                                                                          ln_b, T, C, k);
+  SB_LAUNCH_OK();
+  return SB_OK;
+}
+
+extern "C" int sb_dwconv_bias_silu(const void* x, void* y, const void* w, const float* bias, int32_t batch, int32_t T, int32_t C,
+                                   int32_t k, sb_stream_t stream) {
+  using namespace sb;
+  SB_REQUIRE(x && y && w && bias && batch > 0 && T > 0, SB_EINVAL, "sb_dwconv_bias_silu: bad args");
+  SB_REQUIRE(k == DW2_K && C % 64 == 0 && C <= 1024, SB_ENOSUP, "sb_dwconv_bias_silu: needs k = 31 and C a multiple of 64 up to 1024");
+  const int threads = C / 2;
+  const size_t smem = (size_t)DW2_ROWS * C * 2 + (((size_t)C * DW2_K + 7) & ~(size_t)7) * 2 + (size_t)(threads / 32) * DW2_PASS * 2 * 4 +
+                      DW2_PASS * 2 * 4;
+  static size_t configured = 0;
+  if (smem > configured) {
+    SB_CUDA_OK(cudaFuncSetAttribute(dwconv31_tile_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    configured = smem;
+  }
+  dwconv31_tile_kernel<true><<<dim3((T + DW2_TT - 1) / DW2_TT, batch), threads, smem, (cudaStream_t)stream>>>(
+      (const elem_t*)x, (elem_t*)y, (const elem_t*)w, bias, nullptr, T, C);
   SB_LAUNCH_OK();
   return SB_OK;
 }

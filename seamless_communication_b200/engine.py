@@ -41,6 +41,19 @@ def sinusoid_table(max_len: int, dim: int, legacy_pad_idx: int = 1) -> torch.Ten
     return torch.cat([torch.sin(ang), torch.cos(ang)], dim=1).contiguous()
 
 
+XL_POS_CTX = 4096  # rows n_ctx-1 +- (n_ctx-1) of w2v-BERT v1's relative position table (fairseq2.cpp:622)
+
+
+def relpos_table(n_ctx: int, dim: int) -> torch.Tensor:
+    """RelativePositionalEncoding table of w2v-BERT v1, (2*n_ctx-1, dim) fp32 ([fs2-recall]; DESIGN.md §8): row r encodes
+    the step n_ctx-1-r (rows 0..n_ctx-1: steps n_ctx-1 .. 0, the rest -1 .. -(n_ctx-1)); column 2i holds
+    sin(step * exp(-2i ln(1e4) / dim)), column 2i+1 the cosine.  A checkpoint's `speech_encoder.pos_enc` replaces it."""
+    steps = torch.arange(n_ctx - 1, -n_ctx, -1, dtype=torch.float32)
+    inv = torch.exp(torch.arange(0, dim, 2, dtype=torch.float32) * -(math.log(10000.0) / dim))
+    ang = steps[:, None] * inv[None, :]
+    return torch.stack([torch.sin(ang), torch.cos(ang)], dim=2).reshape(2 * n_ctx - 1, dim).contiguous()
+
+
 def _interleave_glu(w: torch.Tensor) -> torch.Tensor:
     """rows [a_0..a_{M-1}, b_0..b_{M-1}] -> [a_0, b_0, a_1, b_1, ...] (GLU(dim=channels) pairs adjacent)."""
     M = w.shape[0] // 2
@@ -126,6 +139,7 @@ class UnitYEngine:
             lin(name + ".output_proj")
 
         c = self.cfg
+        v1 = c.encoder_variant == "v1"
         if self.has_encoder:
             ln("speech_encoder_frontend.post_extract_layer_norm")
             lin("speech_encoder_frontend.model_dim_proj")
@@ -134,13 +148,34 @@ class UnitYEngine:
             for n in ("ffn1", "ffn2"):
                 ln(f"{p}.{n}_layer_norm"); lin(f"{p}.{n}.inner_proj"); lin(f"{p}.{n}.output_proj")
             ln(f"{p}.self_attn_layer_norm"); mha(f"{p}.self_attn")
-            w[f"{p}.rel_k"] = h(sd[f"{p}.self_attn.sdpa.rel_k_embed.weight"])
+            dw = sd[f"{p}.conv.depthwise_conv.weight"].reshape(c.model_dim, c.dw_kernel)
+            if v1:
+                # u is folded into the q projection's bias (q + u is what multiplies k); the kernel adds v - u for the
+                # positional term.  R = r_proj(pos table) is one GEMM per call (encode_speech).
+                a = sd[f"{p}.self_attn.sdpa.u_bias"].double().reshape(-1)
+                w[f"{p}.self_attn.qkv.b"][:self.M] += a.to(dev, torch.float32)
+                w[f"{p}.r_proj.w"] = h(sd[f"{p}.self_attn.sdpa.r_proj.weight"])
+                w[f"{p}.vu"] = f((sd[f"{p}.self_attn.sdpa.v_bias"].double().reshape(-1) - a).reshape(self.H, -1))
+                # eval BatchNorm folded in fp64: w' = w * g / sqrt(var + eps), bias = beta - mean * g / sqrt(var + eps)
+                bn = f"{p}.conv.batch_norm"
+                scale = sd[bn + ".weight"].double() / torch.sqrt(sd[bn + ".running_var"].double() + 1e-5)
+                w[f"{p}.conv.dw.w"] = h(dw.double() * scale[:, None])
+                w[f"{p}.conv.bn.b"] = f(sd[bn + ".bias"].double() - sd[bn + ".running_mean"].double() * scale)
+            else:
+                w[f"{p}.rel_k"] = h(sd[f"{p}.self_attn.sdpa.rel_k_embed.weight"])
+                w[f"{p}.conv.dw.w"] = h(dw)
+                ln(f"{p}.conv.layer_norm")
             ln(f"{p}.conv_layer_norm")
             conv(f"{p}.conv.pointwise_conv1", glu=True)
-            w[f"{p}.conv.dw.w"] = h(sd[f"{p}.conv.depthwise_conv.weight"].reshape(c.model_dim, c.dw_kernel))
-            ln(f"{p}.conv.layer_norm")
             conv(f"{p}.conv.pointwise_conv2")
             ln(f"{p}.layer_norm")
+        if self.has_encoder and v1:
+            pe = sd.get("speech_encoder.pos_enc")
+            if pe is None:
+                pe = relpos_table(XL_POS_CTX, c.model_dim)
+            elif tuple(pe.shape) != (2 * XL_POS_CTX - 1, c.model_dim):
+                raise ValueError(f"speech_encoder.pos_enc has shape {tuple(pe.shape)}, expected {(2 * XL_POS_CTX - 1, c.model_dim)}")
+            w["relpos"] = h(pe)
         if self.has_encoder:
             ln("speech_encoder.inner_layer_norm"); lin("speech_encoder.proj1"); lin("speech_encoder.proj2")
             p = "speech_encoder.adaptor_layers.0"
@@ -249,6 +284,10 @@ class UnitYEngine:
             fbank = fbank[:, :T2].contiguous()
             lens = torch.clamp(lens, max=T2) if lens is not None else None
         S = T2 // s
+        v1 = c.encoder_variant == "v1"
+        if v1 and S > XL_POS_CTX:  # the relative position table holds distances up to n_ctx - 1
+            raise ValueError(f"The input sequence length must be less than or equal to the maximum sequence length "
+                             f"({XL_POS_CTX}), but is {S} instead.")
         lens_s = (lens // s).to(I32) if lens is not None else None
         x = Seq(B, S, Cf * s, lens=lens_s, buf=fbank.reshape(B * S, Cf * s))
         x = self._ln(x, "speech_encoder_frontend.post_extract_layer_norm")
@@ -256,11 +295,22 @@ class UnitYEngine:
         for i in range(c.enc_layers):
             p = f"speech_encoder.inner.layers.{i}"
             x = self._ffn(self._ln(x, p + ".ffn1_layer_norm"), p + ".ffn1", c.enc_ffn_dim, ACT_SILU, x, alpha=0.5)
-            x = self._mha_self(self._ln(x, p + ".self_attn_layer_norm"), p + ".self_attn", x, rel=self.w[p + ".rel_k"])
+            if v1:
+                # R = r_proj(table rows n_ctx-S .. n_ctx+S-2), shared by the batch; row S-1+j-i encodes distance i-j
+                pos = Seq(1, 2 * S - 1, M, buf=self.w["relpos"][XL_POS_CTX - S:XL_POS_CTX + S - 1])
+                r = self._lin(pos, p + ".r_proj", M)
+                qkv = self._lin(self._ln(x, p + ".self_attn_layer_norm"), p + ".self_attn.qkv", 3 * M)
+                a = ops.self_attention_relpos(qkv, self.H, r.buf, vb=self.w[p + ".vu"])
+                x = self._lin(a, p + ".self_attn.output_proj", M, res1=x)
+            else:
+                x = self._mha_self(self._ln(x, p + ".self_attn_layer_norm"), p + ".self_attn", x, rel=self.w[p + ".rel_k"])
             hcv = self._ln(x, p + ".conv_layer_norm", mask=True)
             g = self._lin(hcv, p + ".conv.pointwise_conv1", 2 * M, glu=True)
-            d = ops.dwconv_ln_silu(g, self.w[p + ".conv.dw.w"], self.w[p + ".conv.layer_norm.w"],
-                                   self.w[p + ".conv.layer_norm.b"], c.dw_kernel)
+            if v1:
+                d = ops.dwconv_bias_silu(g, self.w[p + ".conv.dw.w"], self.w[p + ".conv.bn.b"], c.dw_kernel)
+            else:
+                d = ops.dwconv_ln_silu(g, self.w[p + ".conv.dw.w"], self.w[p + ".conv.layer_norm.w"],
+                                       self.w[p + ".conv.layer_norm.b"], c.dw_kernel)
             x = self._lin(d, p + ".conv.pointwise_conv2", M, res1=x)
             x = self._ffn(self._ln(x, p + ".ffn2_layer_norm"), p + ".ffn2", c.enc_ffn_dim, ACT_SILU, x, alpha=0.5)
             x = self._ln(x, p + ".layer_norm")

@@ -138,6 +138,9 @@ class Translator:
                 sample_rate: int = 16000, unit_generation_ngram_filtering: bool = False, duration_factor: float = 1.0,
                 prosody_encoder_input=None, src_text=None) -> Tuple[List[str], Optional[BatchedSpeechOutput]]:
         input_modality, output_modality = self.get_modalities_from_task_str(task_str)
+        if output_modality == Modality.SPEECH and self.model.config.encoder_variant == "v1":
+            raise NotImplementedError(f"{task_str.upper()} on {self.model.config.name} needs its autoregressive T2U (the "
+                                      "v1 AR T2U model), which is not implemented; S2TT and ASR are")
         if self.apply_mintox and not (src_lang is not None or src_text is not None):
             raise ValueError("`src_lang` must be specified when `apply_mintox` is `True` or you need to specify src_text.")
         if isinstance(input, dict):

@@ -111,7 +111,10 @@ def load_unity_model(name_or_arch: str, device="cuda", dtype=torch.float16, stat
       * `synthetic=True` - seeded random-init weights of the named architecture (synthetic.make_unity_state_dict;
         `seed` and further keywords go there).  Checkpoint URLs are unreachable offline, so tests and benchmarks use this.
     Without any of them a RuntimeError is raised: the reference would download the card's checkpoint, and silently
-    answering with random weights instead would return garbage translations."""
+    answering with random weights instead would return garbage translations.
+
+    A w2v-BERT v1 architecture (`seamlessM4T_large` -> "base") runs speech-to-text only: its T2U (an autoregressive
+    one) and the text encoder are not built, and their keys are dropped from the weights."""
     arch = cfgmod.MODEL_CARDS.get(name_or_arch, name_or_arch)
     if arch not in cfgmod.UNITY_ARCHS:
         raise ValueError(f"unknown model card / architecture '{name_or_arch}'")
@@ -123,17 +126,24 @@ def load_unity_model(name_or_arch: str, device="cuda", dtype=torch.float16, stat
             raise RuntimeError("no tokenizers given: pass tokenizers=(text_tokenizer, char_tokenizer) matching the weights "
                                "(the SentencePiece models of the asset card are not reachable offline), or synthetic=True")
         tokenizers = synthetic_mod.make_tokenizers(cfg)
+    v1 = cfg.encoder_variant == "v1"
     if state_dict is None and checkpoint is not None:
         from ..checkpoint import convert_unity_checkpoint, load_checkpoint_file
         ck = load_checkpoint_file(checkpoint) if isinstance(checkpoint, str) else checkpoint
-        ctok = tokenizers[1]
-        pieces = [ctok.model.index_to_token(i) for i in range(ctok.model.vocabulary_size)]
+        if v1:  # fairseq names of the AR T2U (decoder.*, synthesizer_encoder.*) and of the text encoder
+            ck = {**ck, "model": {k: v for k, v in ck["model"].items()
+                                  if not k.startswith(("decoder.", "synthesizer_encoder.", "text_encoder."))}}
+            pieces = None
+        else:
+            ctok = tokenizers[1]
+            pieces = [ctok.model.index_to_token(i) for i in range(ctok.model.vocabulary_size)]
         state_dict = convert_unity_checkpoint(ck, char_pieces=pieces, nllb_vocab=cfg.text_vocab)["model"]
     if state_dict is None:
         if not synthetic:
             raise RuntimeError(f"no weights for '{name_or_arch}': pass state_dict=..., checkpoint=... (fairseq or fairseq2 naming) "
                                "or synthetic=True for seeded random-init weights; checkpoints cannot be downloaded here")
         state_dict = synthetic_mod.make_unity_state_dict(cfg, seed=seed, with_t2u=with_t2u, **synth_kw)
-    elif not with_t2u:
-        state_dict = {k: v for k, v in state_dict.items() if not k.startswith("t2u_model.")}
+    elif not with_t2u or v1:
+        drop = ("t2u_model.", "text_encoder.", "text_encoder_frontend.") if v1 else ("t2u_model.",)
+        state_dict = {k: v for k, v in state_dict.items() if not k.startswith(drop)}
     return UnitYModel(cfg, UnitYEngine(cfg, state_dict, tokenizers, device=device))

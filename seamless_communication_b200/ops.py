@@ -233,6 +233,35 @@ def self_attention(qkv: Seq, H: int, *, causal=False, rel_k=None, rel_left=0, re
     return out
 
 
+def attention_relpos(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tensor, B, H, S, q_rows, q_halo, kv_rows,
+                     kv_halo, r: torch.Tensor, u=None, vb=None, kv_lens=None):
+    """Transformer-XL relative attention (sb_attention_relpos); r is (2S-1, H*64) fp16, u / vb fp32 (H, 64) or None."""
+    lib = _lib.load()
+    check(lib.sb_attention_relpos(q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0),
+                                  out.data_ptr(), out.stride(0), B, H, S, q_rows, q_halo, kv_rows, kv_halo, _p(kv_lens),
+                                  r.data_ptr(), r.stride(0), _p(u), _p(vb), _stream()), "sb_attention_relpos")
+    return out
+
+
+def self_attention_relpos(qkv: Seq, H: int, r: torch.Tensor, u=None, vb=None) -> Seq:
+    M = qkv.C // 3
+    out = Seq(qkv.B, qkv.T, M, qkv.PH, qkv.Tp, qkv.lens, zero=qkv.PH > 0)
+    b = qkv.buf
+    attention_relpos(b[:, 0:M], b[:, M:2 * M], b[:, 2 * M:3 * M], out.buf, qkv.B, H, qkv.T, qkv.Tp, qkv.PH, qkv.Tp, qkv.PH, r,
+                     u, vb, qkv.lens)
+    return out
+
+
+def dwconv_bias_silu(x: Seq, w, bias, k: int) -> Seq:
+    """w2v-BERT v1 depthwise conv (symmetric padding) + per-channel bias (BatchNorm folded into w) + SiLU."""
+    lib = _lib.load()
+    assert x.PH == 0 and x.Tp == x.T
+    y = x.like()
+    check(lib.sb_dwconv_bias_silu(x.buf.data_ptr(), y.buf.data_ptr(), w.data_ptr(), bias.data_ptr(), x.B, x.T, x.C, k,
+                                  _stream()), "sb_dwconv_bias_silu")
+    return y
+
+
 def dwconv_ln_silu(x: Seq, w, ln_w, ln_b, k: int) -> Seq:
     lib = _lib.load()
     assert x.PH == 0 and x.Tp == x.T

@@ -71,9 +71,17 @@ class _Init:
 def make_unity_state_dict(cfg: UnitYConfig, seed: int = 0, logit_scale: float = 4.0,
                           with_t2u: bool = True, dur_gain: float = 0.02, dur_bias: float = 0.0,
                           embed_scale: float = 0.25, dec_gain: float = 1.0) -> Dict[str, torch.Tensor]:
-    """Random-init UnitY2 parameters under the reference's state_dict names (SURVEY 8b)."""
+    """Random-init UnitY2 parameters under the reference's state_dict names (SURVEY 8b).
+
+    With cfg.encoder_variant == "v1" the Conformer layers carry the w2v-BERT v1 parameters instead of the Shaw table and
+    the conv-module LayerNorm: `self_attn.sdpa.r_proj` (no bias), `u_bias` / `v_bias` (H, 64) and
+    `conv.batch_norm.{weight,bias,running_mean,running_var}` with non-trivial running statistics; no T2U is drawn.
+    The v2 draws, and so every v2 state dict, are unchanged."""
     I = _Init(seed)
     M = cfg.model_dim
+    v1 = cfg.encoder_variant == "v1"
+    if v1:
+        with_t2u = False
     fd = cfg.fbank_channels * cfg.fbank_stride
     I.ln("speech_encoder_frontend.post_extract_layer_norm", fd)
     I.linear("speech_encoder_frontend.model_dim_proj", M, fd)
@@ -85,12 +93,23 @@ def make_unity_state_dict(cfg: UnitYConfig, seed: int = 0, logit_scale: float = 
             I.linear(f"{p}.{f}.output_proj", M, cfg.enc_ffn_dim)
         I.ln(f"{p}.self_attn_layer_norm", M)
         I.mha(f"{p}.self_attn", M)
-        I.normal(f"{p}.self_attn.sdpa.rel_k_embed.weight", (cfg.shaw_left + cfg.shaw_right + 1, cfg.head_dim),
-                 cfg.head_dim ** -0.5)
+        if v1:
+            I.linear(f"{p}.self_attn.sdpa.r_proj", M, M, bias=False)
+            I.normal(f"{p}.self_attn.sdpa.u_bias", (cfg.num_heads, cfg.head_dim), 0.5)
+            I.normal(f"{p}.self_attn.sdpa.v_bias", (cfg.num_heads, cfg.head_dim), 0.5)
+        else:
+            I.normal(f"{p}.self_attn.sdpa.rel_k_embed.weight", (cfg.shaw_left + cfg.shaw_right + 1, cfg.head_dim),
+                     cfg.head_dim ** -0.5)
         I.ln(f"{p}.conv_layer_norm", M)
         I.conv(f"{p}.conv.pointwise_conv1", 2 * M, M, 1, bias=False)
         I.normal(f"{p}.conv.depthwise_conv.weight", (M, 1, cfg.dw_kernel), 1.0 / math.sqrt(cfg.dw_kernel))
-        I.ln(f"{p}.conv.layer_norm", M)
+        if v1:
+            bn = f"{p}.conv.batch_norm"
+            I.ln(bn, M)  # weight around 1, bias around 0
+            I.normal(bn + ".running_mean", (M,), 0.2)
+            I.sd[bn + ".running_var"] = _round_fp16(0.25 + 1.5 * torch.rand(M, generator=I.g))
+        else:
+            I.ln(f"{p}.conv.layer_norm", M)
         I.conv(f"{p}.conv.pointwise_conv2", M, M, 1, bias=False)
         I.ln(f"{p}.layer_norm", M)
     I.ln("speech_encoder.inner_layer_norm", M)
