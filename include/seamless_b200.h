@@ -124,7 +124,9 @@ int sb_fbank(const float* wave, int64_t wave_ld, const int32_t* num_samples, int
 /* ------------------------------------------------------------------------------------------------------------------
  * sb_layernorm - y = LN(x (+ res)) * w + b over the last dim (eps 1e-5), fp16 io, fp32 statistics.
  * Rows are addressed in sequence layout on both sides; rows at positions >= len are written as zeros when
- * mask_out != 0.  Replaces LayerNorm_forward (fairseq2.cpp:266).
+ * mask_out != 0.  res (optional) has x's layout and is added to x in fp32 before the statistics, without rounding;
+ * sum_out (optional, used only with res) receives x + res rounded to fp16 in the OUT layout (out_rows / out_halo).
+ * SB_ENOSUP unless dim is a multiple of 8 and at most 2048.  Replaces LayerNorm_forward (fairseq2.cpp:266).
  * ---------------------------------------------------------------------------------------------------------------- */
 int sb_layernorm(const void* x, const void* res, void* y, void* sum_out, const float* w, const float* b, int32_t dim,
                  int32_t batch, int32_t T, int32_t in_rows, int32_t in_halo, int32_t out_rows, int32_t out_halo,
@@ -132,8 +134,13 @@ int sb_layernorm(const void* x, const void* res, void* y, void* sum_out, const f
 
 /* ------------------------------------------------------------------------------------------------------------------
  * sb_attention - multi-head scaled dot-product attention, head_dim 64, fp16 io, fp32 softmax, flash-style.
- *   scores = (q.k^T + q.rel_k[clamp(j-i,-left,right)+left]) / 8, key mask j < kv_lens[b], optional causal mask.
- * q/k/v/out pointers address row 0 of sequence 0 (sequence layout given by the x_rows / x_halo arguments), x_ld = row stride.
+ *   scores = (q.k^T + q.rel_k[clamp(j-i,-left,right)+left]) / 8, key mask j < kv_lens[b] (kv_lens NULL: j < sk);
+ *   causal != 0 also masks j > i + sk - sq (aligned bottom-right: the last query row sees every key).
+ *   A row with no admissible key (kv_lens[b] == 0, or a causal row i < sq - sk) is written as 0.
+ * q/k/v/out pointers address row 0 of sequence 0 (sequence layout given by the x_rows / x_halo arguments; out uses q's),
+ * x_ld = row stride.  Only rows [q_halo, q_halo + sq) x columns [0, heads*64) of each sequence of out are written.
+ * SB_ENOSUP, before anything is launched: q_ld, k_ld or v_ld not a multiple of 8 elements, out_ld odd, or rel_k != NULL
+ * with left + right + 1 > 80.
  * Replaces MultiheadAttention_forward (fairseq2.cpp:399-499) and ShawRelativePositionSDPA
  * (models/conformer_shaw/builder.py:127-146).
  * ---------------------------------------------------------------------------------------------------------------- */

@@ -159,6 +159,7 @@ __global__ void __launch_bounds__(DW_THREADS) dwconv_ln_silu_fixed_kernel(const 
 //     one warp per frame; nothing but the staged input ever round-trips shared memory.
 // fp32 FMA bound: 0.5 GFMA per layer = 16 us at 132 SMs x 128 lanes (H100 SXM, data-sheet clock).
 constexpr int DW2_TT = 32, DW2_PASS = 16, DW2_K = 31, DW2_ROWS = DW2_TT + DW2_K - 1;
+constexpr int DW2_RED = 3;  // per (warp, frame) partial statistics: sum, sum of squares, sum of squares about the warp's mean
 
 __device__ __forceinline__ void dw_cp_async16(void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
@@ -173,9 +174,9 @@ __global__ void __launch_bounds__(512) dwconv31_tile_kernel(const elem_t* __rest
   extern __shared__ __align__(16) uint8_t smem_dw[];
   elem_t* sx = reinterpret_cast<elem_t*>(smem_dw);                                   // [62][C]
   elem_t* sw = sx + (size_t)DW2_ROWS * C;                                            // [C][31] as in global memory
-  float* red = reinterpret_cast<float*>(sw + (((size_t)C * DW2_K + 7) & ~(size_t)7)); // [warps][16][2]
+  float* red = reinterpret_cast<float*>(sw + (((size_t)C * DW2_K + 7) & ~(size_t)7)); // [warps][16][DW2_RED]
   const int nwarp = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  float* stat = red + (size_t)nwarp * DW2_PASS * 2;                                  // [16][2] mean, rstd
+  float* stat = red + (size_t)nwarp * DW2_PASS * DW2_RED;                            // [16][2] mean, rstd
   const int b = blockIdx.y, t0 = blockIdx.x * DW2_TT;
   const elem_t* xb = x + (long long)b * T * C;
   const int vec_per_row = C / 8;
@@ -237,22 +238,40 @@ __global__ void __launch_bounds__(512) dwconv31_tile_kernel(const elem_t* __rest
       }
       continue;
     }
-    // LayerNorm statistics of the 16 frames over all channels
+    // LayerNorm statistics of the 16 frames over all channels.  var = E[a^2] - mean^2 in fp32 is accurate while |mean| is a
+    // few sd and loses the variance from |mean| ~ 100 sd on; there the per-warp sums of squares about each warp's own mean
+    // (64 channels) are combined instead, with the parallel-variance formula M2 = sum_w M2_w + 64 sum_w (mean_w - mean)^2.
+    // Frames with |mean| <= 8 sd keep E[a^2] - mean^2 bit for bit (its error there is ~1e-5 of the variance).
 #pragma unroll
     for (int t = 0; t < DW2_PASS; ++t) {
       const float s = warp_sum(acc[t].x + acc[t].y);
       const float q = warp_sum(acc[t].x * acc[t].x + acc[t].y * acc[t].y);
-      if (lane == 0) { red[((size_t)warp * DW2_PASS + t) * 2] = s; red[((size_t)warp * DW2_PASS + t) * 2 + 1] = q; }
+      const float mw = s * (1.f / 64.f);
+      const float dx = acc[t].x - mw, dy = acc[t].y - mw;
+      const float m2 = warp_sum(dx * dx + dy * dy);
+      if (lane == 0) {
+        float* r = red + ((size_t)warp * DW2_PASS + t) * DW2_RED;
+        r[0] = s; r[1] = q; r[2] = m2;
+      }
     }
     __syncthreads();
     for (int f = warp; f < DW2_PASS; f += nwarp) {  // one warp per frame (fewer warps than frames when C < 1024)
       float s = 0.f, q = 0.f;
-      for (int i = lane; i < nwarp; i += 32) { s += red[((size_t)i * DW2_PASS + f) * 2]; q += red[((size_t)i * DW2_PASS + f) * 2 + 1]; }
+      for (int i = lane; i < nwarp; i += 32) { s += red[((size_t)i * DW2_PASS + f) * DW2_RED]; q += red[((size_t)i * DW2_PASS + f) * DW2_RED + 1]; }
       s = warp_sum(s); q = warp_sum(q);
+      const float mean = s / C;
+      float m2 = 0.f;  // every lane takes part in the shuffles; lane 0 decides which variance to keep
+      for (int i = lane; i < nwarp; i += 32) {
+        const float* r = red + ((size_t)i * DW2_PASS + f) * DW2_RED;
+        const float d = r[0] * (1.f / 64.f) - mean;
+        m2 += r[2] + 64.f * d * d;
+      }
+      m2 = warp_sum(m2);
       if (lane == 0) {
-        const float mean = s / C;
+        const float e2 = q / C;
+        const float var1 = __fsub_rn(e2, __fmul_rn(mean, mean));  // rounded twice, not fused: the established statistics
         stat[f * 2] = mean;
-        stat[f * 2 + 1] = rsqrtf(fmaxf(q / C - mean * mean, 0.f) + 1e-5f);
+        stat[f * 2 + 1] = e2 > 65.f * var1 ? rsqrtf(m2 / C + 1e-5f) : rsqrtf(fmaxf(var1, 0.f) + 1e-5f);
       }
     }
     __syncthreads();
@@ -283,7 +302,7 @@ extern "C" int sb_dwconv_ln_silu(const void* x, void* y, const void* w, const fl
     static int tile_ok = -1;
     if (tile_ok < 0) { const char* e = getenv("SB_DWCONV_TILE"); tile_ok = (e == nullptr || atoi(e) != 0) ? 1 : 0; }
     const int threads = C / 2, nwarp = threads / 32;
-    const size_t smem2 = (size_t)DW2_ROWS * C * 2 + (((size_t)C * DW2_K + 7) & ~(size_t)7) * 2 + (size_t)nwarp * DW2_PASS * 2 * 4 + DW2_PASS * 2 * 4;
+    const size_t smem2 = (size_t)DW2_ROWS * C * 2 + (((size_t)C * DW2_K + 7) & ~(size_t)7) * 2 + (size_t)nwarp * DW2_PASS * DW2_RED * 4 + DW2_PASS * 2 * 4;
     if (tile_ok && smem2 <= 220 * 1024) {
       static size_t configured2 = 0;
       if (smem2 > configured2) {
@@ -330,7 +349,7 @@ extern "C" int sb_dwconv_bias_silu(const void* x, void* y, const void* w, const 
   SB_REQUIRE(x && y && w && bias && batch > 0 && T > 0, SB_EINVAL, "sb_dwconv_bias_silu: bad args");
   SB_REQUIRE(k == DW2_K && C % 64 == 0 && C <= 1024, SB_ENOSUP, "sb_dwconv_bias_silu: needs k = 31 and C a multiple of 64 up to 1024");
   const int threads = C / 2;
-  const size_t smem = (size_t)DW2_ROWS * C * 2 + (((size_t)C * DW2_K + 7) & ~(size_t)7) * 2 + (size_t)(threads / 32) * DW2_PASS * 2 * 4 +
+  const size_t smem = (size_t)DW2_ROWS * C * 2 + (((size_t)C * DW2_K + 7) & ~(size_t)7) * 2 + (size_t)(threads / 32) * DW2_PASS * DW2_RED * 4 +
                       DW2_PASS * 2 * 4;
   static size_t configured = 0;
   if (smem > configured) {
