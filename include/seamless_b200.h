@@ -97,7 +97,9 @@ int sb_gemm_skinny(const sb_gemm_t* g, int32_t splits, float* partials, int64_t 
  * MMA A operand and all rows are the B operand, so a CTA reads its weights once and the activations once per k-block
  * (the row-major kernel re-reads a 128-row activation tile for every 64 features and is L2 -> SM bound at 160 rows).
  * partials != NULL: split-K mode, same output contract as sb_gemm_splitk (splits need not divide the k-blocks).
- * partials == NULL (splits must be 1): out = act(a . w^T + bias) in fp16, act in {none, relu}. */
+ * partials == NULL (splits must be 1): out = act(a . w^T + bias) in fp16, act in {none, relu}.  At splits that divide
+ * the k-blocks the partials are bit-identical to sb_gemm_splitk's and sb_gemm_skinny's on the H100 (same k-blocks in
+ * the same m64 x k16 steps; tests/test_decode_gemm.py checks it), so the decoder step's outputs do not depend on the path. */
 int sb_gemm_decode_supported(const sb_gemm_t* g, int32_t splits);
 int sb_gemm_decode(const sb_gemm_t* g, int32_t splits, float* partials, int64_t slice_rows, sb_stream_t stream);
 /* consumer of the partials: x += bias + sum_z partial[z] (x fp16 [rows][dim], updated in place) and h = LayerNorm(x).

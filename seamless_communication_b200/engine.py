@@ -93,10 +93,9 @@ class UnitYEngine:
         # costs about as much as a kernel boundary inside a CUDA graph, so the fusion saves launches but not waiting.
         self.decode_fused = os.environ.get("SB_DECODER_FUSED", "0") != "0"
         self.decode_timeline = os.environ.get("SB_DS_TIMELINE", "0") != "0"
-        # SB_DECODE_GEMM_T=1: q|k|v / FFN products of the decoder step on the transposed wgmma kernel (decode_gemm.cu).
-        # Opt-in (not timed on H100): it moves 2.6x fewer bytes through L2, but at these sizes the launches are bound by
-        # fixed latencies rather than by L2 traffic.
-        self.decode_gemm_t = os.environ.get("SB_DECODE_GEMM_T", "0") != "0"
+        # all six weight products of a decoder step on the transposed wgmma kernel (decode_gemm.cu) at <= 256 rows;
+        # SB_DECODE_GEMM_T=0 selects the row-major wgmma + mma.sync skinny chain instead
+        self.decode_gemm_t = os.environ.get("SB_DECODE_GEMM_T", "1") != "0"
         self.topk_tiles = os.environ.get("SB_TOPK_TILES", "1") != "0"  # top-K from the projection's per-tile statistics
 
     # ------------------------------------------------------------------------------------------ weight packing
@@ -380,18 +379,20 @@ class UnitYEngine:
                                           st["step"].data_ptr(), st["ML"], st["att"].buf.data_ptr(), R, H, stream),
                   "sb_decode_self_attn")
             ops.gemm_splitk(st["att"], w[p + ".self_attn.output_proj.w"], M, S_ATT, part,
-                            prefetch=w[p + ".encoder_decoder_attn.q_proj.w"] if pf else None, skinny=sk["attn"])
+                            prefetch=w[p + ".encoder_decoder_attn.q_proj.w"] if pf else None, skinny=sk["attn"],
+                            transposed=st["gemm_t"])
             ops.splitk_reduce_ln(part, S_ATT, w[p + ".self_attn.output_proj.b"], x, w[p + ".encoder_decoder_attn_layer_norm.w"],
                                  w[p + ".encoder_decoder_attn_layer_norm.b"], h)
             ops.gemm_splitk(h, w[p + ".encoder_decoder_attn.q_proj.w"], M, S_ATT, part,
-                            prefetch=w[p + ".encoder_decoder_attn.output_proj.w"] if pf else None, skinny=sk["attn"])
+                            prefetch=w[p + ".encoder_decoder_attn.output_proj.w"] if pf else None, skinny=sk["attn"],
+                            transposed=st["gemm_t"])
             kv = st["cross_kv"][i].buf
             check(lib.sb_decode_cross_attn(None, part.data_ptr(), S_ATT, SR, w[p + ".encoder_decoder_attn.q_proj.b"].data_ptr(),
                                            kv.data_ptr(), kv[:, M:].data_ptr(), kv.stride(0), ops._p(st["enc_lens"]),
                                            st["S_enc"], st["att"].buf.data_ptr(), R, st["beam"], H, stream),
                   "sb_decode_cross_attn")
             ops.gemm_splitk(st["att"], w[p + ".encoder_decoder_attn.output_proj.w"], M, S_ATT, part,
-                            prefetch=w[p + ".ffn.inner_proj.w"] if pf else None, skinny=sk["attn"])
+                            prefetch=w[p + ".ffn.inner_proj.w"] if pf else None, skinny=sk["attn"], transposed=st["gemm_t"])
             ops.splitk_reduce_ln(part, S_ATT, w[p + ".encoder_decoder_attn.output_proj.b"], x, w[p + ".ffn_layer_norm.w"],
                                  w[p + ".ffn_layer_norm.b"], h)
             if st["gemm_t"]:
@@ -495,13 +496,10 @@ class UnitYEngine:
         while k_att % st["splits_qkv"]: st["splits_qkv"] -= 1
         while k_att % st["splits_attn"]: st["splits_attn"] -= 1
         while k_ffn % st["splits_ffn"]: st["splits_ffn"] -= 1
-        # <= 256 rows: q|k|v, FFN inner and FFN output run on the transposed wgmma kernel (decode_gemm.cu: the row-major
-        # kernel is L2 -> SM bound at these shapes); one (128-feature tile, K slice) unit per CTA, splits fill the machine
+        # <= 256 rows: all six products run on the transposed wgmma kernel (decode_gemm.cu: the row-major kernel is
+        # L2 -> SM bound at these shapes).  It takes the same K slices as the chain above: every slice then sums the
+        # same k-blocks in the same order, so both paths produce the same partials and the same search.
         st["gemm_t"] = self.decode_gemm_t and R <= 256 and M % 64 == 0 and c.dec_ffn_dim % 64 == 0
-        if st["gemm_t"]:
-            sms = torch.cuda.get_device_properties(dev).multi_processor_count
-            st["splits_qkv"] = max(1, min(k_att // 2, sms // ((3 * M + 127) // 128)))
-            st["splits_ffn"] = max(1, min(k_ffn // 4, 16, sms // ((M + 127) // 128)))
         st["part_qkv"] = torch.empty((st["splits_qkv"] * ops.slice_rows(R), 3 * M), dtype=torch.float32, device=dev)
         st["partials"] = torch.empty((max(st["splits_attn"], st["splits_ffn"]) * ops.slice_rows(R), M), dtype=torch.float32,
                                      device=dev)

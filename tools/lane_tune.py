@@ -10,14 +10,15 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+CHAIN = dict(decode_gemm_t=False)  # the skinny choices apply to the row-major chain only
 CONFIGS = [
     ("base", {}),
-    ("gemm_t", dict(decode_gemm_t=True)),
-    ("skinny attn+qkv", dict(skinny_sites={"attn", "qkv"})),
-    ("skinny attn+ffn2", dict(skinny_sites={"attn", "ffn2"})),
-    ("skinny all", dict(skinny_sites={"attn", "qkv", "ffn1", "ffn2"})),
-    ("attn splits 4", dict(skinny_splits=(4, 4, 16))),
-    ("attn splits 16", dict(skinny_splits=(4, 16, 16))),
+    ("chain", CHAIN),
+    ("chain skinny attn+qkv", dict(CHAIN, skinny_sites={"attn", "qkv"})),
+    ("chain skinny attn+ffn2", dict(CHAIN, skinny_sites={"attn", "ffn2"})),
+    ("chain skinny all", dict(CHAIN, skinny_sites={"attn", "qkv", "ffn1", "ffn2"})),
+    ("chain attn splits 4", dict(CHAIN, skinny_splits=(4, 4, 16))),
+    ("chain attn splits 16", dict(CHAIN, skinny_splits=(4, 16, 16))),
     ("no prefetch", dict(decode_prefetch=False)),
 ]
 
