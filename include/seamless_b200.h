@@ -86,20 +86,13 @@ int sb_gemm(const sb_gemm_t* g, sb_stream_t stream);
  * products to rows [z*slice_rows, z*slice_rows + m) of `partials` (row stride n; slice_rows a multiple of 128 enables
  * the TMA-store epilogue).  Only a/w/shape fields of `g` are used. */
 int sb_gemm_splitk(const sb_gemm_t* g, int32_t splits, float* partials, int64_t slice_rows, sb_stream_t stream);
-/* The same products for at most 160 rows (one decoder step of 32 sentences x beam 5) on a short-latency kernel
- * (cp.async + mma.sync, skinny_gemm.cu) instead of the TMA/wgmma pipeline, whose fixed set-up cost dominates at this
- * size.  partials != NULL: split-K mode, same output contract as sb_gemm_splitk.  partials == NULL (splits must be 1):
- * out = act(a . w^T + bias) in fp16, act in {none, relu}.  sb_gemm_skinny_supported returns 1 when the shape qualifies
- * (taps 1, m <= 160, n % 64 == 0, c_in % (64 * splits) == 0, 16-byte aligned operands). */
-int sb_gemm_skinny_supported(const sb_gemm_t* g, int32_t splits);
-int sb_gemm_skinny(const sb_gemm_t* g, int32_t splits, float* partials, int64_t slice_rows, sb_stream_t stream);
 /* The same products for at most 256 rows in TRANSPOSED form on wgmma (decode_gemm.cu): a 128-feature weight tile is the
  * MMA A operand and all rows are the B operand, so a CTA reads its weights once and the activations once per k-block
  * (the row-major kernel re-reads a 128-row activation tile for every 64 features and is L2 -> SM bound at 160 rows).
  * partials != NULL: split-K mode, same output contract as sb_gemm_splitk (splits need not divide the k-blocks).
  * partials == NULL (splits must be 1): out = act(a . w^T + bias) in fp16, act in {none, relu}.  At splits that divide
- * the k-blocks the partials are bit-identical to sb_gemm_splitk's and sb_gemm_skinny's on the H100 (same k-blocks in
- * the same m64 x k16 steps; tests/test_decode_gemm.py checks it), so the decoder step's outputs do not depend on the path. */
+ * the k-blocks the partials are bit-identical to sb_gemm_splitk's on the H100 (same k-blocks in the same m64 x k16
+ * steps; tests/test_decode_gemm.py checks it), so the decoder step's outputs do not depend on the path. */
 int sb_gemm_decode_supported(const sb_gemm_t* g, int32_t splits);
 int sb_gemm_decode(const sb_gemm_t* g, int32_t splits, float* partials, int64_t slice_rows, sb_stream_t stream);
 /* consumer of the partials: x += bias + sum_z partial[z] (x fp16 [rows][dim], updated in place) and h = LayerNorm(x).

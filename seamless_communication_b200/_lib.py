@@ -88,8 +88,6 @@ PROTOTYPES = {
     "sb_gemm": [C.POINTER(GemmDesc), c_p],
     "sb_gemm_ref": [C.POINTER(GemmDesc), c_p],
     "sb_gemm_splitk": [C.POINTER(GemmDesc), i32, c_p, i64, c_p],
-    "sb_gemm_skinny_supported": [c_p, i32],
-    "sb_gemm_skinny": [c_p, i32, c_p, i64, c_p],
     "sb_gemm_decode_supported": [c_p, i32],
     "sb_gemm_decode": [c_p, i32, c_p, i64, c_p],
     "sb_splitk_reduce_ln": [c_p, i32, i32, i64, i32, c_p, c_p, c_p, c_p, c_p, c_p],

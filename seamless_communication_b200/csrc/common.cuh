@@ -61,9 +61,9 @@ int sm_count();  // SMs of the current device (cached per device)
 // 2D fp16 (esize 2) / fp32 (esize 4) tensor map: inner = channels, box 128 B x box_rows, 128B swizzle, OOB -> 0 (gemm_tcgen05.cu)
 int make_tmap(CUtensorMap* tm, const void* base, uint64_t inner, uint64_t rows, uint64_t ld_elems, uint32_t box_rows,
               int esize = 2);
-// sb_gemm with tile_stats at <= 256 rows on the weight-stationary projection kernel (vocab_proj.cu)
-bool vocab_proj_supported(const sb_gemm_t* g);
-int vocab_proj(const sb_gemm_t* g, cudaStream_t st);
+// sb_gemm with tile_stats at <= 256 rows on the weight-stationary projection kernel (decode_gemm.cu).  Returns false,
+// launching nothing, when the shape does not qualify; else true with the launch's status in *rc.
+bool vocab_proj(const sb_gemm_t* g, cudaStream_t st, int* rc);
 
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {

@@ -654,31 +654,6 @@ __global__ void __launch_bounds__(DS_THREADS, 2) decoder_step_kernel(const __gri
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-int encode_map(CUtensorMap* tm, const void* base, uint64_t inner, uint64_t rows, uint32_t box_rows) {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-  }
-  SB_REQUIRE(fn != nullptr, SB_ECUDA, "cuTensorMapEncodeTiled entry point not available");
-  cuuint64_t dims[2] = {inner, rows};
-  cuuint64_t strides[1] = {inner * 2};
-  cuuint32_t box[2] = {(cuuint32_t)DS_BK, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  SB_REQUIRE(r == CUDA_SUCCESS, SB_ECUDA, "sb_decoder_plan: cuTensorMapEncodeTiled failed (%d) inner=%llu rows=%llu box_rows=%u",
-             (int)r, (unsigned long long)inner, (unsigned long long)rows, box_rows);
-  return SB_OK;
-}
-
 typedef void (*DsKernel)(DsParams);
 DsKernel pick_kernel(int npad) {
   switch (npad) {
@@ -834,11 +809,11 @@ extern "C" int sb_decoder_plan_init(const sb_decoder_plan_desc_t* d, sb_decoder_
   P->part_qkv = d->part_qkv; P->part = d->part; P->hist = (elem_t*)d->hist;
   P->counters = d->counters; P->timeline = (unsigned long long*)d->timeline;
   DsParams& maps = *P;
-  if ((rc = encode_map(&maps.h, d->h, (uint64_t)d->dim, (uint64_t)d->rows, (uint32_t)info.npad))) return fail(rc);
-  if ((rc = encode_map(&maps.att, d->att, (uint64_t)d->dim, (uint64_t)d->rows, (uint32_t)info.npad))) return fail(rc);
-  if ((rc = encode_map(&maps.t, d->ffn_act, (uint64_t)d->ffn_dim, (uint64_t)d->rows, (uint32_t)info.npad))) return fail(rc);
-  if ((rc = encode_map(&maps.w_dim, d->w_dim_stack, (uint64_t)d->dim, (uint64_t)d->layers * (6ull * d->dim + d->ffn_dim), DS_TM))) return fail(rc);
-  if ((rc = encode_map(&maps.w_ffn, d->w_ffn_stack, (uint64_t)d->ffn_dim, (uint64_t)d->layers * d->dim, DS_TM))) return fail(rc);
+  if ((rc = make_tmap(&maps.h, d->h, (uint64_t)d->dim, (uint64_t)d->rows, (uint64_t)d->dim, (uint32_t)info.npad))) return fail(rc);
+  if ((rc = make_tmap(&maps.att, d->att, (uint64_t)d->dim, (uint64_t)d->rows, (uint64_t)d->dim, (uint32_t)info.npad))) return fail(rc);
+  if ((rc = make_tmap(&maps.t, d->ffn_act, (uint64_t)d->ffn_dim, (uint64_t)d->rows, (uint64_t)d->ffn_dim, (uint32_t)info.npad))) return fail(rc);
+  if ((rc = make_tmap(&maps.w_dim, d->w_dim_stack, (uint64_t)d->dim, (uint64_t)d->layers * (6ull * d->dim + d->ffn_dim), (uint64_t)d->dim, DS_TM))) return fail(rc);
+  if ((rc = make_tmap(&maps.w_ffn, d->w_ffn_stack, (uint64_t)d->ffn_dim, (uint64_t)d->layers * d->dim, (uint64_t)d->ffn_dim, DS_TM))) return fail(rc);
   for (int l = 0; l < d->layers; ++l) {
     const sb_decoder_layer_t& s = d->layer[l];
     DsLayer& L = P->layer[l];

@@ -607,10 +607,11 @@ extern "C" int sb_gemm(const sb_gemm_t* g_in, sb_stream_t stream) {
   auto tiles = [&](int bn) { return mt * ((g->n + bn - 1) / bn); };
   if (g->tile_stats != nullptr) {
     SB_REQUIRE(!g->glu && g->n >= 128, SB_ENOSUP, "sb_gemm: tile_stats needs n >= 128 and no GLU");
-    // up to 256 rows (a beam-search step): the weight-stationary kernel of vocab_proj.cu, which reads each weight row once.
+    // up to 256 rows (a beam-search step): the weight-stationary kernel of decode_gemm.cu, which reads each weight row once.
     // SB_PROJ_T=0 selects the general kernel (read per call: tools compare both inside one process)
     const char* ep = getenv("SB_PROJ_T");
-    if ((ep == nullptr || atoi(ep) != 0) && sb::vocab_proj_supported(g)) return sb::vocab_proj(g, st);
+    int rc = SB_OK;
+    if ((ep == nullptr || atoi(ep) != 0) && sb::vocab_proj(g, st, &rc)) return rc;
     return sb::launch<128>(g, st);  // the statistics are per 128-column tile (SB_STATS_TILE)
   }
   // 256-wide tiles for the large products (encoder / T2U / vocoder GEMMs): fp16 single-output epilogues, whole tiles only

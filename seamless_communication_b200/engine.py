@@ -84,9 +84,6 @@ class UnitYEngine:
         self._state_lock = threading.RLock()
         self.search_groups = 1  # concurrent sentence groups in beam_search (see _search_group_count)
         self.decode_prefetch = os.environ.get("SB_DECODE_PREFETCH", "1") != "0"
-        self.decode_skinny = os.environ.get("SB_DECODE_SKINNY", "1") != "0"  # <= 160 rows: skinny_gemm.cu
-        self.skinny_splits = tuple(int(v) for v in os.environ.get("SB_SKINNY_SPLITS", "4,8,16").split(","))  # qkv, attn, ffn2
-        self.skinny_sites = set(os.environ.get("SB_SKINNY_SITES", "attn").split(","))  # of qkv, attn, ffn1, ffn2
         self.graph_kernels = 0  # kernels executed through CUDA-graph replays (bench.py: gpu_launches)
         # SB_DECODER_FUSED=1: one persistent kernel per decoder step (sb_decoder_step, csrc/decoder_step.cu) instead of the
         # per-op launch chain.  Opt-in (correct and deterministic, not timed on H100): a grid-wide phase barrier through L2
@@ -94,7 +91,7 @@ class UnitYEngine:
         self.decode_fused = os.environ.get("SB_DECODER_FUSED", "0") != "0"
         self.decode_timeline = os.environ.get("SB_DS_TIMELINE", "0") != "0"
         # all six weight products of a decoder step on the transposed wgmma kernel (decode_gemm.cu) at <= 256 rows;
-        # SB_DECODE_GEMM_T=0 selects the row-major wgmma + mma.sync skinny chain instead
+        # SB_DECODE_GEMM_T=0 selects the row-major wgmma chain instead
         self.decode_gemm_t = os.environ.get("SB_DECODE_GEMM_T", "1") != "0"
         self.topk_tiles = os.environ.get("SB_TOPK_TILES", "1") != "0"  # top-K from the projection's per-tile statistics
 
@@ -364,7 +361,6 @@ class UnitYEngine:
                                 self.pos.data_ptr(), math.sqrt(M), x.buf.data_ptr(), R, M, stream), "sb_embed_step")
         self._ln(x, "text_decoder.layers.0.self_attn_layer_norm", out=h)
         S_ATT, S_FFN, S_QKV, SR = st["splits_attn"], st["splits_ffn"], st["splits_qkv"], ops.slice_rows(R)
-        sk = st["skinny"]
         pf = self.decode_prefetch  # each GEMM pulls the weights of the GEMM after it into L2 (latency-bound chain)
         for i in range(c.dec_layers):
             p = f"text_decoder.layers.{i}"
@@ -373,39 +369,33 @@ class UnitYEngine:
             w_next = None if last else w[f"text_decoder.layers.{i + 1}.self_attn.qkv.w"]
             # qkv / q projections also run split-K; their partials are reduced (+bias) inside the attention kernels
             ops.gemm_splitk(h, w[p + ".self_attn.qkv.w"], 3 * M, S_QKV, st["part_qkv"],
-                            prefetch=w[p + ".self_attn.output_proj.w"] if pf else None, skinny=sk["qkv"], transposed=st["gemm_t"])
+                            prefetch=w[p + ".self_attn.output_proj.w"] if pf else None, transposed=st["gemm_t"])
             check(lib.sb_decode_self_attn(None, st["part_qkv"].data_ptr(), S_QKV, SR, w[p + ".self_attn.qkv.b"].data_ptr(),
                                           st["kc"][i].data_ptr(), st["vc"][i].data_ptr(), st["anc"].data_ptr(), st["ML"],
                                           st["step"].data_ptr(), st["ML"], st["att"].buf.data_ptr(), R, H, stream),
                   "sb_decode_self_attn")
             ops.gemm_splitk(st["att"], w[p + ".self_attn.output_proj.w"], M, S_ATT, part,
-                            prefetch=w[p + ".encoder_decoder_attn.q_proj.w"] if pf else None, skinny=sk["attn"],
-                            transposed=st["gemm_t"])
+                            prefetch=w[p + ".encoder_decoder_attn.q_proj.w"] if pf else None, transposed=st["gemm_t"])
             ops.splitk_reduce_ln(part, S_ATT, w[p + ".self_attn.output_proj.b"], x, w[p + ".encoder_decoder_attn_layer_norm.w"],
                                  w[p + ".encoder_decoder_attn_layer_norm.b"], h)
             ops.gemm_splitk(h, w[p + ".encoder_decoder_attn.q_proj.w"], M, S_ATT, part,
-                            prefetch=w[p + ".encoder_decoder_attn.output_proj.w"] if pf else None, skinny=sk["attn"],
-                            transposed=st["gemm_t"])
+                            prefetch=w[p + ".encoder_decoder_attn.output_proj.w"] if pf else None, transposed=st["gemm_t"])
             kv = st["cross_kv"][i].buf
             check(lib.sb_decode_cross_attn(None, part.data_ptr(), S_ATT, SR, w[p + ".encoder_decoder_attn.q_proj.b"].data_ptr(),
                                            kv.data_ptr(), kv[:, M:].data_ptr(), kv.stride(0), ops._p(st["enc_lens"]),
                                            st["S_enc"], st["att"].buf.data_ptr(), R, st["beam"], H, stream),
                   "sb_decode_cross_attn")
             ops.gemm_splitk(st["att"], w[p + ".encoder_decoder_attn.output_proj.w"], M, S_ATT, part,
-                            prefetch=w[p + ".ffn.inner_proj.w"] if pf else None, skinny=sk["attn"], transposed=st["gemm_t"])
+                            prefetch=w[p + ".ffn.inner_proj.w"] if pf else None, transposed=st["gemm_t"])
             ops.splitk_reduce_ln(part, S_ATT, w[p + ".encoder_decoder_attn.output_proj.b"], x, w[p + ".ffn_layer_norm.w"],
                                  w[p + ".ffn_layer_norm.b"], h)
             if st["gemm_t"]:
                 t = ops.gemm_decode(h, w[p + ".ffn.inner_proj.w"], c.dec_ffn_dim, w[p + ".ffn.inner_proj.b"], act=ACT_RELU,
                                     out=st["ffn"], prefetch=w[p + ".ffn.output_proj.w"] if pf else None)
-            elif sk["ffn1"]:
-                t = ops.gemm_skinny(h, w[p + ".ffn.inner_proj.w"], c.dec_ffn_dim, w[p + ".ffn.inner_proj.b"], act=ACT_RELU,
-                                    out=st["ffn"], prefetch=w[p + ".ffn.output_proj.w"] if pf else None)
             else:
                 t = self._lin(h, p + ".ffn.inner_proj", c.dec_ffn_dim, act=ACT_RELU, out=st["ffn"],
                               prefetch=w[p + ".ffn.output_proj.w"] if pf else None)
-            ops.gemm_splitk(t, w[p + ".ffn.output_proj.w"], M, S_FFN, part, prefetch=w_next if pf else None,
-                            skinny=sk["ffn2"], transposed=st["gemm_t"])
+            ops.gemm_splitk(t, w[p + ".ffn.output_proj.w"], M, S_FFN, part, prefetch=w_next if pf else None, transposed=st["gemm_t"])
             ops.splitk_reduce_ln(part, S_FFN, w[p + ".ffn.output_proj.b"], x, w[nxt + ".w"], w[nxt + ".b"], h)
         check(lib.sb_store_step(h.buf.data_ptr(), st["hist"].data_ptr(), st["step"].data_ptr(), R * M * 2, stream), "sb_store_step")
         ops.gemm(h, w["text_embed"], c.text_vocab, None, out=st["logits"], out_f32=True, tile_stats=st["tile_stats"])
@@ -476,29 +466,10 @@ class UnitYEngine:
         st["vc"] = [torch.empty((ML, R, M), dtype=F16, device=dev) for _ in range(c.dec_layers)]
         for name, width in (("x", M), ("h", M), ("q", M), ("att", M), ("qkv", 3 * M), ("ffn", c.dec_ffn_dim)):
             st[name] = Seq(1, R, width)
-        k_att, k_ffn = max(M // 64, 1), max(c.dec_ffn_dim // 64, 1)  # k-blocks of the two residual GEMM kinds
-        st["splits_attn"] = max(1, min(4, k_att // 4))
-        st["splits_ffn"] = max(1, min(8, k_ffn // 8))
-        st["splits_qkv"] = max(1, min(2, k_att // 8))
-        # at <= 160 rows the 1024 x 1024 projections of a step (self/cross attention out, cross q) run on the
-        # short-latency mma.sync kernel (skinny_gemm.cu) with more, smaller K slices (tools/skinny_bench.py times both).
-        # The wider products stay on the wgmma GEMM (mma.sync runs out of tensor throughput there).  SB_SKINNY_SITES
-        # overrides.
-        ok = self.decode_skinny and R <= 160 and M % 64 == 0 and c.dec_ffn_dim % 64 == 0
-        st["skinny"] = {site: ok and site in self.skinny_sites for site in ("qkv", "attn", "ffn1", "ffn2")}
-        sq, sa, sf = self.skinny_splits
-        if st["skinny"]["qkv"]:
-            st["splits_qkv"] = max(1, min(sq, k_att))
-        if st["skinny"]["attn"]:
-            st["splits_attn"] = max(1, min(sa, k_att))
-        if st["skinny"]["ffn2"]:
-            st["splits_ffn"] = max(1, min(sf, k_ffn))
-        while k_att % st["splits_qkv"]: st["splits_qkv"] -= 1
-        while k_att % st["splits_attn"]: st["splits_attn"] -= 1
-        while k_ffn % st["splits_ffn"]: st["splits_ffn"] -= 1
+        st["splits_qkv"], st["splits_attn"], st["splits_ffn"] = ops.decode_splits(R, M, c.dec_ffn_dim)
         # <= 256 rows: all six products run on the transposed wgmma kernel (decode_gemm.cu: the row-major kernel is
-        # L2 -> SM bound at these shapes).  It takes the same K slices as the chain above: every slice then sums the
-        # same k-blocks in the same order, so both paths produce the same partials and the same search.
+        # L2 -> SM bound at these shapes).  It takes the same K slices as the row-major chain: every slice then
+        # sums the same k-blocks in the same order, so both paths produce the same partials and the same search.
         st["gemm_t"] = self.decode_gemm_t and R <= 256 and M % 64 == 0 and c.dec_ffn_dim % 64 == 0
         st["part_qkv"] = torch.empty((st["splits_qkv"] * ops.slice_rows(R), 3 * M), dtype=torch.float32, device=dev)
         st["partials"] = torch.empty((max(st["splits_attn"], st["splits_ffn"]) * ops.slice_rows(R), M), dtype=torch.float32,

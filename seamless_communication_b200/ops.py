@@ -134,24 +134,21 @@ def hifigan_resblock(x: Seq, w1, b1, w2, b2, k: int, dil, *, res2: Optional[Seq]
     return out
 
 
-def gemm_skinny(a: Seq, w: torch.Tensor, n: int, bias=None, *, act=ACT_NONE, out: Seq,
-                prefetch: Optional[torch.Tensor] = None) -> Seq:
-    """out = act(a @ w.T + bias) for a dense Seq of at most 160 rows on the short-latency kernel (skinny_gemm.cu)."""
-    lib = _lib.load()
-    assert a.PH == 0 and a.Tp == a.T and out.PH == 0 and out.Tp == out.T
-    d = GemmDesc()
-    d.a, d.a_rows, d.a_ld, d.c_in, d.taps, d.dil, d.a_row0 = a.buf.data_ptr(), a.B * a.T, a.buf.stride(0), a.C, 1, 1, 0
-    d.w, d.n, d.m = w.data_ptr(), n, a.B * a.T
-    d.bias, d.act, d.alpha, d.gamma = _p(bias), act, 1.0, 1.0
-    d.out, d.out_ld = out.buf.data_ptr(), out.buf.stride(0)
-    if prefetch is not None:
-        d.prefetch, d.prefetch_bytes = prefetch.data_ptr(), prefetch.numel() * prefetch.element_size()
-    check(lib.sb_gemm_skinny(C.byref(d), 1, None, 0, _stream()), "sb_gemm_skinny")
-    return out
-
-
-def gemm_skinny_supported(rows: int, n: int, k: int, splits: int = 1) -> bool:
-    return rows <= 160 and n % 64 == 0 and k % (64 * splits) == 0
+def decode_splits(rows: int, dim: int, ffn_dim: int) -> tuple:
+    """K slices (q|k|v, the three dim x dim attention products, FFN out) of the split-K products of a decoder step of
+    `rows` rows, on the transposed kernel and on the row-major chain alike.  The slices fix the fp32 summation order
+    and with it the search's results, so any change to them is a change of outputs."""
+    k_att, k_ffn = max(dim // 64, 1), max(ffn_dim // 64, 1)  # k-blocks of the two residual GEMM kinds
+    qkv = max(1, min(2, k_att // 8))
+    if rows <= 160 and dim % 64 == 0 and ffn_dim % 64 == 0:
+        attn = max(1, min(8, k_att))
+    else:
+        attn = max(1, min(4, k_att // 4))
+    ffn = max(1, min(8, k_ffn // 8))
+    while k_att % qkv: qkv -= 1
+    while k_att % attn: attn -= 1
+    while k_ffn % ffn: ffn -= 1
+    return qkv, attn, ffn
 
 
 def slice_rows(rows: int) -> int:
@@ -160,7 +157,7 @@ def slice_rows(rows: int) -> int:
 
 
 def gemm_splitk(a: Seq, w: torch.Tensor, n: int, splits: int, partials: torch.Tensor,
-                prefetch: Optional[torch.Tensor] = None, skinny=False, transposed=False) -> None:
+                prefetch: Optional[torch.Tensor] = None, transposed=False) -> None:
     """Raw fp32 partial products of a (dense) Seq against w into partials[(z*slice_rows(rows) + r), n]."""
     lib = _lib.load()
     assert a.PH == 0 and a.Tp == a.T
@@ -172,9 +169,6 @@ def gemm_splitk(a: Seq, w: torch.Tensor, n: int, splits: int, partials: torch.Te
         d.prefetch, d.prefetch_bytes = prefetch.data_ptr(), prefetch.numel() * prefetch.element_size()
     if transposed and lib.sb_gemm_decode_supported(C.byref(d), splits):
         check(lib.sb_gemm_decode(C.byref(d), splits, partials.data_ptr(), slice_rows(a.B * a.T), _stream()), "sb_gemm_decode")
-        return
-    if skinny and lib.sb_gemm_skinny_supported(C.byref(d), splits):
-        check(lib.sb_gemm_skinny(C.byref(d), splits, partials.data_ptr(), slice_rows(a.B * a.T), _stream()), "sb_gemm_skinny")
         return
     check(lib.sb_gemm_splitk(C.byref(d), splits, partials.data_ptr(), slice_rows(a.B * a.T), _stream()), "sb_gemm_splitk")
 

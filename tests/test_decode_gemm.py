@@ -1,12 +1,14 @@
 """decode_gemm.cu (sb_gemm_decode, the transposed wgmma kernel behind all six weight products of a beam-search step)
 against float64 at every decoder-step shape of seamlessM4T_large, at the row counts the searches run (160 = 32 x beam 5,
 40 = the s2tt batch of 8 x 5, and ragged ones), at the splits a step uses, one split and an uneven split; bit for bit
-against the row-major and skinny kernels at the step's splits; and one whole search on the default (transposed) path
-against the row-major launch chain."""
+against the row-major kernels at the step's splits; and one whole search on the default (transposed) path against the
+row-major launch chain."""
 import math
 
 import pytest
 import torch
+
+from seamless_communication_b200.ops import decode_splits
 
 pytestmark = pytest.mark.gpu
 dev = "cuda"
@@ -30,9 +32,13 @@ def _operands(rows, n, k, seed):
     return a, w, bias, ref
 
 
-# K splits of a seamlessM4T_large step (engine._search_state): q|k|v 2, the 1024 x 1024 products 8 (skinny kernel on the
-# row-major chain at <= 160 rows, else 4), FFN out 8
-STEP_SPLITS = {(3 * M, M): 2, (M, M): 8, (M, FFN): 8}
+def step_splits(rows):
+    """K splits of a seamlessM4T_large step of `rows` rows (engine._search_state), per (n, k) product"""
+    qkv, attn, ffn = decode_splits(rows, M, FFN)
+    return {(3 * M, M): qkv, (M, M): attn, (M, FFN): ffn}
+
+
+STEP_SPLITS = step_splits(160)  # the bench step's splits, which the float64 tests try at every row count
 
 
 def _split_choices(n, k):
@@ -85,19 +91,16 @@ def test_direct_bias_relu_matches_float64(ops, rows, n, k):
 
 
 @pytest.mark.parametrize("rows", ROWS)
-def test_bit_identical_to_row_major_chain(ops, rows):
+def test_bit_identical_to_row_major_kernels_at_step_slices(ops, rows):
     """At the step's K slices the transposed kernel sums the same k-blocks in the same order as the kernels of the
-    row-major chain (sb_gemm_splitk, sb_gemm_skinny for the 1024 x 1024 products at <= 160 rows, sb_gemm for FFN
-    inner), so its partials and its fp16 FFN output are bit-identical to theirs and a search does not depend on the
-    path."""
+    row-major chain (sb_gemm_splitk, sb_gemm for FFN inner), so its partials and its fp16 FFN output are bit-identical
+    to theirs and a search does not depend on the path."""
     from seamless_communication_b200.ops import Seq
     SR = ops.slice_rows(rows)
-    for (n, k), splits in STEP_SPLITS.items():
-        skinny = (n, k) == (M, M) and rows <= 160
-        splits = splits if (n, k) != (M, M) or skinny else 4
+    for (n, k), splits in step_splits(rows).items():
         a, w, _, _ = _operands(rows, n, k, rows * 13 + n + k)
         want, got = (torch.zeros(splits * SR, n, device=dev) for _ in range(2))
-        ops.gemm_splitk(a, w, n, splits, want, skinny=skinny)
+        ops.gemm_splitk(a, w, n, splits, want)
         ops.gemm_splitk(a, w, n, splits, got, transposed=True)
         assert torch.equal(got.view(splits, SR, n)[:, :rows], want.view(splits, SR, n)[:, :rows]), (n, k, splits)
     a, w, bias, _ = _operands(rows, FFN, M, rows * 17)
@@ -108,7 +111,7 @@ def test_bit_identical_to_row_major_chain(ops, rows):
 
 def test_search_step_transposed_equals_launch_chain():
     """A beam search of 32 sentences x beam 5 (160 rows, the bench's step) on `small`: the default path (all six products
-    on sb_gemm_decode) against decode_gemm_t = False (row-major + skinny chain), at the same K slices: the hypotheses,
+    on sb_gemm_decode) against decode_gemm_t = False (the row-major chain), at the same K slices: the hypotheses,
     their scores and the final-LayerNorm state of every step are identical; and a second default search is too."""
     from seamless_communication_b200.models.unity import load_unity_model
     from seamless_communication_b200.ops import Seq

@@ -264,6 +264,17 @@ def test_synthetic_assets_follow_reference_layout():
            (1024, 24, 24, 256102, 10082, 10943)
 
 
+def test_decode_splits_keep_the_step_slices():
+    """The K slices of a decoder step's split-K products fix its fp32 sums and so its search results: q|k|v, the three
+    model_dim x model_dim products and FFN out, for the 1024 / 8192 models (base, base_v2, small_*) and tiny_* (128 / 256)."""
+    from seamless_communication_b200.ops import decode_splits
+    want = {(1024, 8192): {5: (2, 8, 8), 40: (2, 8, 8), 160: (2, 8, 8), 161: (2, 4, 8), 256: (2, 4, 8), 257: (2, 4, 8)},
+            (128, 256): {5: (1, 2, 1), 40: (1, 2, 1), 160: (1, 2, 1), 161: (1, 1, 1), 256: (1, 1, 1), 257: (1, 1, 1)}}
+    for (dim, ffn), by_rows in want.items():
+        for rows, splits in by_rows.items():
+            assert decode_splits(rows, dim, ffn) == splits, (dim, ffn, rows)
+
+
 def test_shard_bounds_cover_batch():
     for n, w in ((256, 8), (33, 4), (3, 8)):
         spans = [shard_bounds(n, w, r) for r in range(w)]

@@ -1,7 +1,7 @@
-"""The weight-stationary vocabulary projection (vocab_proj.cu): sb_gemm with tile_stats at <= 256 rows.  Its logits and
-per-tile log-softmax statistics must equal those of the general kernel (SB_PROJ_T=0) bit for bit, since a last-bit change
-in a row's log-sum-exp shifts every candidate of the row and can flip a cross-beam near tie, and agree with the CUDA-core
-reference kernel within fp32 summation-order noise."""
+"""The weight-stationary vocabulary projection (vocab_proj_kernel in decode_gemm.cu): sb_gemm with tile_stats at <= 256
+rows.  Its logits and per-tile log-softmax statistics must equal those of the general kernel (SB_PROJ_T=0) bit for
+bit, since a last-bit change in a row's log-sum-exp shifts every candidate of the row and can flip a cross-beam near
+tie, and agree with the CUDA-core reference kernel within fp32 summation-order noise."""
 import math
 import os
 

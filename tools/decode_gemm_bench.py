@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-launch time of the six weight products of one decoder layer at the bench's beam-search step shape (160 rows,
-seamlessM4T_large: model 1024, FFN 8192), on the launch chain (row-major wgmma + skinny mma.sync) and on the transposed
-kernel (sb_gemm_decode) at each split count it can take, plus the split-K reduction that follows a residual product.
+seamlessM4T_large: model 1024, FFN 8192), on the row-major launch chain (sb_gemm_splitk at the step's K slices, sb_gemm
+for FFN inner) and on the transposed kernel (sb_gemm_decode) at each split count it can take, plus the split-K reduction that follows a residual product.
 Each CUDA graph chains launches over 24 different weight tensors, so weights come from HBM as in a step.
 Prints the card and its power limit with the numbers."""
 import argparse
@@ -24,6 +24,7 @@ args = ap.parse_args()
 R, LAYERS, REPS, M, FFN = args.rows, 24, 4, 1024, 8192
 dev = "cuda"
 SPLITS = [int(s) for s in args.splits.split(",")]
+S_QKV, S_ATT, S_FFN = ops.decode_splits(R, M, FFN)
 
 
 def timed(fn):
@@ -59,8 +60,7 @@ def product(name, n, k, chain, direct=False):
     if chain == "tc_direct":
         res.append(("chain tc", timed(lambda i: ops.gemm(a, ws[i], n, bias, act=ops.ACT_RELU, out=out))))
     else:
-        kind, sp = chain
-        res.append((f"chain {kind}/{sp}", timed(lambda i: ops.gemm_splitk(a, ws[i], n, sp, part, skinny=kind == "sk"))))
+        res.append((f"chain splitk/{chain}", timed(lambda i: ops.gemm_splitk(a, ws[i], n, chain, part))))
     if direct:
         res.append(("T direct", timed(lambda i: ops.gemm_decode(a, ws[i], n, bias, act=ops.ACT_RELU, out=out))))
     for sp in SPLITS:
@@ -84,10 +84,10 @@ def reduce_ln():
 card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                       capture_output=True, text=True).stdout.strip()
 print(f"card: {card}\nrows {R}, per launch (in-graph, 24 distinct weights); TB/s = weight bytes / time")
-product("q|k|v", 3 * M, M, ("tc", 2))
-product("self-attn out", M, M, ("sk", 8))
-product("cross q", M, M, ("sk", 8))
-product("cross out", M, M, ("sk", 8))
+product("q|k|v", 3 * M, M, S_QKV)
+product("self-attn out", M, M, S_ATT)
+product("cross q", M, M, S_ATT)
+product("cross out", M, M, S_ATT)
 product("FFN inner", FFN, M, "tc_direct", direct=True)
-product("FFN out", M, FFN, ("tc", 8))
+product("FFN out", M, FFN, S_FFN)
 reduce_ln()

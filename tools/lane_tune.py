@@ -1,4 +1,4 @@
-"""Decoder-step kernel choices (skinny sites / split counts / transposed wgmma / L2 prefetch) timed with 1 and with
+"""Decoder-step kernel choices (transposed wgmma or the row-major chain / L2 prefetch) timed with 1 and with
 `--lanes` beam searches in flight: under lanes the cheapest choice in SM-slot time wins, not the shortest latency chain.
 Usage: python tools/lane_tune.py [--lanes 4]"""
 import argparse
@@ -10,15 +10,9 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-CHAIN = dict(decode_gemm_t=False)  # the skinny choices apply to the row-major chain only
 CONFIGS = [
     ("base", {}),
-    ("chain", CHAIN),
-    ("chain skinny attn+qkv", dict(CHAIN, skinny_sites={"attn", "qkv"})),
-    ("chain skinny attn+ffn2", dict(CHAIN, skinny_sites={"attn", "ffn2"})),
-    ("chain skinny all", dict(CHAIN, skinny_sites={"attn", "qkv", "ffn1", "ffn2"})),
-    ("chain attn splits 4", dict(CHAIN, skinny_splits=(4, 4, 16))),
-    ("chain attn splits 16", dict(CHAIN, skinny_splits=(4, 16, 16))),
+    ("chain", dict(decode_gemm_t=False)),
     ("no prefetch", dict(decode_prefetch=False)),
 ]
 
@@ -38,7 +32,7 @@ def main():
     waves = S.make_waveforms(32, bench.SAMPLES, seed=1234).to(device)
     enc, _ = eng.encode_speech(tr.fbank_batch(waves)["seqs"], None)
     prefix = [eng.cfg.text_eos, eng.text_tokenizer.lang_index(bench.TGT_LANG)]
-    defaults = {k: getattr(eng, k) for k in ("decode_gemm_t", "skinny_sites", "skinny_splits", "decode_prefetch")}
+    defaults = {k: getattr(eng, k) for k in ("decode_gemm_t", "decode_prefetch")}
     pool1, poolL = LanePool(device, 1, [eng]), LanePool(device, a.lanes, [eng])
     ref = None
     for name, cfg in CONFIGS:

@@ -25,7 +25,7 @@ def main():
     R, M, F, V, H, ML, B, S_ENC, BEAM = 160, 1024, 8192, 256206, 16, 102, 32, 63, 5
     g = torch.Generator(device=dev).manual_seed(0)
     rnd = lambda *s: (torch.randn(*s, device=dev, generator=g) * 0.05).half()  # noqa: E731
-    w_qkv, w_o, w_1, w_2, emb = rnd(3 * M, M), rnd(M, M), rnd(F, M), rnd(M, F), rnd(V, M)
+    w_qkv, w_1, w_2, emb = rnd(3 * M, M), rnd(F, M), rnd(M, F), rnd(V, M)
     b_f, b_m = torch.zeros(F, device=dev), torch.zeros(M, device=dev)
     ln_w, ln_b = torch.ones(M, device=dev), torch.zeros(M, device=dev)
     SR = ops.slice_rows(R)
@@ -49,9 +49,6 @@ def main():
             "qkv  wgmma split 2": lambda: ops.gemm_splitk(d["h"], w_qkv, 3 * M, 2, d["part_qkv"]),
             "ffn1 wgmma direct": lambda: ops.gemm(d["h"], w_1, F, b_f, act=ACT_RELU, out=d["ffn"]),
             "ffn2 wgmma split 8": lambda: ops.gemm_splitk(d["ffn"], w_2, M, 8, d["part"]),
-            "out  skinny split 8": lambda: ops.gemm_splitk(d["att"], w_o, M, 8, d["part"], skinny=True),
-            "qkv  skinny split 4": lambda: ops.gemm_splitk(d["h"], w_qkv, 3 * M, 4, d["part_qkv"], skinny=True),
-            "ffn2 skinny split 16": lambda: ops.gemm_splitk(d["ffn"], w_2, M, 16, d["part"], skinny=True),
             "reduce + LayerNorm": lambda: ops.splitk_reduce_ln(d["part"], 8, b_m, d["x"], ln_w, ln_b, d["h"]),
             "self attention t=50": lambda: _lib.check(lib.sb_decode_self_attn(
                 None, d["part_qkv"].data_ptr(), 2, SR, zero_bias.data_ptr(), d["kc"].data_ptr(), d["vc"].data_ptr(),
