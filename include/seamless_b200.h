@@ -227,6 +227,9 @@ typedef struct {
   int32_t* fin_count; float* fin_score; int32_t* fin_len; int32_t* fin_seqs; int32_t* active;
   int32_t* fin_anc;    /* [B][beam][max_len] or NULL: per finished hypothesis, the cache slot of every position */
   int32_t* n_active;   /* [1] number of sentences still searching (written every step) */
+  const int32_t* len_budget; /* [1] on the device or NULL: the search's length budget (<= max_len; EOS forced at step
+                                budget-2, no step past budget-1), so one captured step serves every budget up to the
+                                allocated max_len, which stays the row stride of the arrays above.  NULL: max_len */
 } sb_beam_t;
 int sb_beam_step(const sb_beam_t* p, sb_stream_t stream);
 

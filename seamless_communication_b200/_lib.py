@@ -44,7 +44,7 @@ class BeamDesc(C.Structure):
         ("cand_val", c_p), ("cand_idx", c_p), ("eos_lprob", c_p),
         ("seqs", c_p), ("scores", c_p), ("anc", c_p),
         ("fin_count", c_p), ("fin_score", c_p), ("fin_len", c_p), ("fin_seqs", c_p), ("active", c_p),
-        ("fin_anc", c_p), ("n_active", c_p),
+        ("fin_anc", c_p), ("n_active", c_p), ("len_budget", c_p),
     ]
 
 

@@ -12,7 +12,9 @@ Named architectures:
     the parity tests so the CPU oracle finishes in seconds;
   * ``base``     - seamlessM4T_large (builder.py:109-134, w2v-BERT v1 speech
     encoder, same 600m / dense_1b dims), with ``tiny_v1`` / ``small_v1`` test
-    copies.  Only speech-to-text runs on them: they carry no T2U.
+    copies.  Their T2U is the autoregressive one (t2u_builder.py:141-160
+    `_base_t2u`): a pre-LN Transformer encoder and an NLLB-type decoder over the
+    unit vocabulary, sized by the same ``t2u_*`` / ``unit_*`` fields.
 """
 from __future__ import annotations
 
@@ -45,16 +47,24 @@ _VOCODER_FIRST_SPKR = [0, 1, 2, 3, 4, 6, 7, 9, 10, 11, 14, 15, 16, 17, 29, 30, 3
                        44, 45, 46, 49, 52, 53, 54, 61, 62, 63, 66, 69]
 
 
-def vocoder_lang_spkr_idx_map() -> Dict[str, Dict]:
+# first speaker id per language of cards/vocoder_36langs.yaml (seamlessM4T_large's vocoder; same 36 languages in the
+# same order, different speaker table: tests/golden/vocoder_36langs_map.json holds the card's whole map)
+_VOCODER36_FIRST_SPKR = [0, 2, 3, 4, 5, 6, 7, 9, 10, 11, 14, 15, 16, 17, 29, 30, 31, 32, 35, 36, 37, 38, 39, 40, 41,
+                         42, 43, 46, 49, 50, 51, 58, 59, 60, 63, 66]
+
+
+def vocoder_lang_spkr_idx_map(card: str = "vocoder_v2") -> Dict[str, Dict]:
+    first = _VOCODER36_FIRST_SPKR if card == "vocoder_36langs" else _VOCODER_FIRST_SPKR
     return {
         "multilingual": {l: i for i, l in enumerate(VOCODER_LANGS_V2)},
-        "multispkr": {l: [_VOCODER_FIRST_SPKR[i]] for i, l in enumerate(VOCODER_LANGS_V2)},
+        "multispkr": {l: [first[i]] for i, l in enumerate(VOCODER_LANGS_V2)},
     }
 
 
 @dataclass
 class UnitYConfig:
-    """Flat config of the whole S2ST stack (speech encoder, text decoder, NAR T2U)."""
+    """Flat config of the whole S2ST stack (speech encoder, text decoder, T2U).  The T2U is non-autoregressive for
+    encoder_variant "v2" and autoregressive for "v1" (seamlessM4T_large)."""
 
     name: str = "base_v2"
     model_dim: int = 1024
@@ -81,14 +91,17 @@ class UnitYConfig:
     text_unk: int = 1
     text_bos: int = 2
     text_eos: int = 3
-    # --- NAR T2U ("base_nar") ---
+    # --- T2U: NAR "base_nar" (v2) or AR "base" (v1, t2u_builder.py:141-160); both 6 + 6 layers, FFN 8192 ---
     t2u_enc_layers: int = 6
     t2u_dec_layers: int = 6
     t2u_ffn_dim: int = 8192
-    unit_vocab: int = 10082
+    unit_vocab: int = 10082  # AR: num_units + 2 * (len(unit_langs) + 1) + 4
     num_units: int = 10000
     unit_pad: int = 1
     unit_eos: int = 2
+    unit_bos: int = 0
+    unit_unk: int = 3
+    unit_max_seq_len: int = 2048  # position table of the AR T2U decoder
     char_vocab: int = 10943
     char_pad: int = 1
     fft_kernel: int = 7
@@ -184,7 +197,7 @@ def small_v2() -> UnitYConfig:
 
 
 def base() -> UnitYConfig:
-    """seamlessM4T_large: the base_v2 dims with the w2v-BERT v1 encoder; speech-to-text only here (no T2U)."""
+    """seamlessM4T_large: the base_v2 dims with the w2v-BERT v1 encoder and the autoregressive T2U."""
     return UnitYConfig(name="base", encoder_variant="v1")
 
 
@@ -221,7 +234,7 @@ UNITY_ARCHS = {"base_v2": base_v2, "tiny_v2": tiny_v2, "small_v2": small_v2, "ba
 VOCODER_ARCHS = {"base": base_vocoder, "tiny": tiny_vocoder}
 
 # asset-card names the reference resolves through fairseq2's asset store
-# (cards/seamlessM4T_v2_large.yaml: model_arch base_v2; cards/vocoder_v2.yaml: base)
+# (cards/seamlessM4T_v2_large.yaml: model_arch base_v2; cards/vocoder_v2.yaml and vocoder_36langs.yaml: base)
 MODEL_CARDS = {"seamlessM4T_v2_large": "base_v2", "seamlessM4T_v2_tiny": "tiny_v2", "seamlessM4T_v2_small": "small_v2",
                "seamlessM4T_large": "base"}
-VOCODER_CARDS = {"vocoder_v2": "base", "vocoder_v2_tiny": "tiny"}
+VOCODER_CARDS = {"vocoder_v2": "base", "vocoder_v2_tiny": "tiny", "vocoder_36langs": "base"}

@@ -751,13 +751,14 @@ __global__ void __launch_bounds__(TKT_THREADS) logits_topk_tiles_kernel(const fl
 __global__ void __launch_bounds__(128) beam_step_kernel(const sb_beam_t p) {
   pdl_sync();
   const int b = blockIdx.x;
-  const int beam = p.beam, K = p.K, ML = p.max_len;
+  const int beam = p.beam, K = p.K, ML = p.max_len;  // ML: row stride of the state arrays
   const int step = *p.step_ptr;
+  const int budget = p.len_budget != nullptr ? min(*p.len_budget, ML) : ML;
   __shared__ int s_parent[16];
   __shared__ int s_tok[16];
   __shared__ float s_score[16];
   __shared__ int s_active;
-  if (step + 1 >= ML) return;  // search exhausted (graph replays beyond the last step are no-ops)
+  if (step + 1 >= budget) return;  // search exhausted (graph replays beyond the last step are no-ops)
   if (threadIdx.x == 0) {
     int active = p.active[b];
     if (active) {
@@ -766,7 +767,7 @@ __global__ void __launch_bounds__(128) beam_step_kernel(const sb_beam_t p) {
       int used[16];
       bool forced_taken[16];
       for (int i = 0; i < nsrc; ++i) { used[i] = 0; forced_taken[i] = false; }
-      const bool force_eos = (step == ML - 2);   // _tweak_lprobs fairseq2.cpp:1280-1291
+      const bool force_eos = (step == budget - 2);  // _tweak_lprobs fairseq2.cpp:1280-1291
       const bool block_eos = (step < p.min_len); // fairseq2.cpp:1273-1278
       int n_ongoing = 0, fin = p.fin_count[b];
       const int want = 2 * beam;

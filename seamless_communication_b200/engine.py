@@ -68,7 +68,10 @@ class UnitYEngine:
         self.text_tokenizer, self.char_tokenizer = tokenizers
         self.M, self.H = cfg.model_dim, cfg.num_heads
         assert cfg.head_dim == 64, "attention kernels are specialised for head_dim 64"
-        self.has_t2u = any(k.startswith("t2u_model.") for k in state_dict)
+        # the NAR T2U (v2) is recognised by its character embedding; an autoregressive T2U (v1) has none, and only its
+        # encoder is packed here (its decoder runs on a decoder-only engine of its own, models/unity/model.py)
+        self.has_t2u = "t2u_model.decoder_frontend.embed_char.weight" in state_dict
+        self.has_t2u_encoder = "t2u_model.encoder.layer_norm.weight" in state_dict
         self.has_encoder = any(k.startswith("speech_encoder.") for k in state_dict)  # a monotonic text decoder has none
         self._pack(state_dict)
         self.pos = sinusoid_table(cfg.max_seq_len, self.M).to(self.device)
@@ -203,12 +206,13 @@ class UnitYEngine:
                 r += t.shape[0]
             self.dec_w_ffn[i * M_:(i + 1) * M_].copy_(w[p + ".ffn.output_proj.w"])
             w[p + ".ffn.output_proj.w"] = self.dec_w_ffn[i * M_:(i + 1) * M_]
-        if self.has_t2u:
+        if self.has_t2u_encoder:
             for i in range(c.t2u_enc_layers):
                 p = f"t2u_model.encoder.layers.{i}"
                 ln(f"{p}.self_attn_layer_norm"); mha(f"{p}.self_attn")
                 ln(f"{p}.ffn_layer_norm"); lin(f"{p}.ffn.inner_proj"); lin(f"{p}.ffn.output_proj")
             ln("t2u_model.encoder.layer_norm")
+        if self.has_t2u:
             P = "t2u_model.decoder_frontend"
             w["unit_embed"] = h(sd[P + ".embed.weight"])
             w["char_embed"] = h(sd[P + ".embed_char.weight"])
@@ -462,6 +466,7 @@ class UnitYEngine:
         st["anc"] = torch.zeros((R, ML), dtype=I32, device=dev)
         st["anc_init"] = torch.arange(R, dtype=I32, device=dev)[:, None].repeat(1, ML).contiguous()
         st["step"] = torch.zeros(1, dtype=I32, device=dev)
+        st["budget"] = torch.full((1,), ML, dtype=I32, device=dev)  # this search's length budget (<= ML), set per search
         st["kc"] = [torch.empty((ML, R, M), dtype=F16, device=dev) for _ in range(c.dec_layers)]
         st["vc"] = [torch.empty((ML, R, M), dtype=F16, device=dev) for _ in range(c.dec_layers)]
         for name, width in (("x", M), ("h", M), ("q", M), ("att", M), ("qkv", 3 * M), ("ffn", c.dec_ffn_dim)):
@@ -495,7 +500,7 @@ class UnitYEngine:
         d.seqs, d.scores, d.anc = st["seqs"].data_ptr(), st["scores"].data_ptr(), st["anc"].data_ptr()
         d.fin_count, d.fin_score, d.fin_len = fin["count"].data_ptr(), fin["score"].data_ptr(), fin["len"].data_ptr()
         d.fin_seqs, d.active, d.n_active = fin["seqs"].data_ptr(), fin["active"].data_ptr(), fin["n_active"].data_ptr()
-        d.fin_anc = fin["anc"].data_ptr()
+        d.fin_anc, d.len_budget = fin["anc"].data_ptr(), st["budget"].data_ptr()
         st["beam_desc"] = d
         st["ds_launch"] = self._decoder_plan(st) if self.decode_fused else None
         st["g_fwd"] = st["g_sel"] = None
@@ -625,10 +630,12 @@ class UnitYEngine:
         fin["n_active"].fill_(st["B"])
         st["step"].zero_()
 
-    def _search_prepare(self, st, enc: Seq, enc_lens, prefix, len_penalty, unk_penalty, min_seq_len, use_graph):
-        """(Re)initialise one cached search state in place for the sentences of `enc`; capture its graphs if needed."""
+    def _search_prepare(self, st, enc: Seq, enc_lens, prefix, len_penalty, unk_penalty, min_seq_len, use_graph, max_len):
+        """(Re)initialise one cached search state in place for the sentences of `enc` and a length budget `max_len`
+        (<= the state's allocated length); capture its graphs if needed."""
         c, M = self.cfg, self.M
         st["unk_penalty"] = float(unk_penalty)
+        st["budget"].fill_(max_len)
         d = st["beam_desc"]
         if st.get("opts_cap") != (min_seq_len, float(len_penalty)) or st.get("unk_cap") != float(unk_penalty):
             d.min_len, d.len_penalty = min_seq_len, len_penalty
@@ -707,11 +714,12 @@ class UnitYEngine:
 
     @torch.inference_mode()
     def beam_search(self, enc: Seq, enc_lens, prefix: List[int], beam=5, soft_max=(1, 200), hard_max=1024,
-                    len_penalty=1.0, unk_penalty=0.0, min_seq_len=1, use_graph=True, cross_kv=None):
+                    len_penalty=1.0, unk_penalty=0.0, min_seq_len=1, use_graph=True, cross_kv=None, state_len=None):
         """Device-resident beam search (see _beam_search); runs on the thread's high-priority stream, ordered after the
         caller's stream on entry and before it on exit."""
         hp = self._priority_stream()
-        args = (enc, enc_lens, prefix, beam, soft_max, hard_max, len_penalty, unk_penalty, min_seq_len, use_graph, cross_kv)
+        args = (enc, enc_lens, prefix, beam, soft_max, hard_max, len_penalty, unk_penalty, min_seq_len, use_graph, cross_kv,
+                state_len)
         if hp is None:
             return self._beam_search(*args)
         cur = torch.cuda.current_stream()
@@ -722,10 +730,13 @@ class UnitYEngine:
         return out
 
     def _beam_search(self, enc: Seq, enc_lens, prefix: List[int], beam=5, soft_max=(1, 200), hard_max=1024,
-                     len_penalty=1.0, unk_penalty=0.0, min_seq_len=1, use_graph=True, cross_kv=None):
+                     len_penalty=1.0, unk_penalty=0.0, min_seq_len=1, use_graph=True, cross_kv=None, state_len=None):
         """Device-resident beam search.  Returns per sentence the finished hypotheses [(score, ids)], best first
         (semantics: fairseq2.cpp:1371-1608; see decode.cu).  `cross_kv` is ignored (kept for API stability): the
-        static cross-attention K/V of the cached search state are recomputed from `enc`."""
+        static cross-attention K/V of the cached search state are recomputed from `enc`.
+        `state_len`: allocate (and cache) the search state for this many positions instead of the length budget
+        min(hard_max, a*S_enc + b); the budget is then a device scalar of the state, so searches whose budgets differ
+        share one state and its captured graphs.  None: the state is sized by the budget."""
         M = self.M
         B, S_enc = enc.B, enc.T
         a, b = soft_max
@@ -736,6 +747,7 @@ class UnitYEngine:
             raise ValueError(f"The input sequence length must be less than or equal to the maximum sequence length "
                              f"({self.cfg.max_seq_len}), but is {ML} instead.")
         assert enc.PH == 0 and enc.Tp == enc.T, "encoder output must be a halo-free Seq"
+        ML_state = ML if state_len is None else max(ML, int(state_len))
         G = self._search_group_count(B)
         bounds = [(B * g) // G for g in range(G + 1)]
         main = torch.cuda.current_stream()
@@ -744,10 +756,10 @@ class UnitYEngine:
         groups = []
         for g in range(G):
             b0, b1 = bounds[g], bounds[g + 1]
-            st = self._search_state(b1 - b0, S_enc, ML, beam, P, enc_lens is not None, use_graph, slot=g)
+            st = self._search_state(b1 - b0, S_enc, ML_state, beam, P, enc_lens is not None, use_graph, slot=g)
             e = enc if G == 1 else Seq(b1 - b0, S_enc, M, buf=enc.buf[b0 * S_enc:b1 * S_enc])
             self._search_prepare(st, e, None if enc_lens is None else enc_lens[b0:b1], prefix, len_penalty, unk_penalty,
-                                 min_seq_len, use_graph)
+                                 min_seq_len, use_graph, ML)
             st["b0"] = b0
             groups.append(st)
         n_steps = ML - 1 - (P - 1)
@@ -844,6 +856,17 @@ class UnitYEngine:
 
     # ------------------------------------------------------------------------------------------ a11-a14 NAR T2U
     @torch.inference_mode()
+    def t2u_encode(self, x: Seq) -> Seq:
+        """The T2U's pre-LN Transformer encoder over the text decoder states (UnitYNART2UModel.encode, model.py:404-412,
+        and UnitYT2UModel.encode, :292-298), keys masked by x.lens."""
+        c = self.cfg
+        for i in range(c.t2u_enc_layers):
+            p = f"t2u_model.encoder.layers.{i}"
+            x = self._mha_self(self._ln(x, p + ".self_attn_layer_norm"), p + ".self_attn", x)
+            x = self._ffn(self._ln(x, p + ".ffn_layer_norm"), p + ".ffn", c.t2u_ffn_dim, ACT_RELU, x)
+        return self._ln(x, "t2u_model.encoder.layer_norm")
+
+    @torch.inference_mode()
     def t2u(self, dec_out: Seq, text_seqs: torch.Tensor, duration_factor: float = 1.0,
             durations: Optional[torch.Tensor] = None):
         """UnitYNART2UModel.forward (model.py:379-402) + argmax/pad/UnitTokenDecoder (generator.py:338-353).
@@ -852,12 +875,7 @@ class UnitYEngine:
         c, M, dev = self.cfg, self.M, self.device
         B, L = dec_out.B, dec_out.T
         stream = ops._stream()
-        x = dec_out
-        for i in range(c.t2u_enc_layers):
-            p = f"t2u_model.encoder.layers.{i}"
-            x = self._mha_self(self._ln(x, p + ".self_attn_layer_norm"), p + ".self_attn", x)
-            x = self._ffn(self._ln(x, p + ".ffn_layer_norm"), p + ".ffn", c.t2u_ffn_dim, ACT_RELU, x)
-        t2u_enc = self._ln(x, "t2u_model.encoder.layer_norm")
+        t2u_enc = self.t2u_encode(dec_out)
         # --- NARDecoderFrontend (nar_decoder_frontend.py:300-334)
         ts = text_seqs.to(I32).contiguous()
         max_c = (L - 2) * self.max_chars + 1 if L > 2 else 1
@@ -1012,7 +1030,35 @@ class VocoderEngine:
         = hop*T_b; durations (B,U) int32 on the device).  `durations` (B,U) replaces the predicted ones (as
         VarianceAdaptor.forward(durations=...) does for the T2U)."""
         x0, lens, tot, dur = self._expand(units, lang_idx, spkr_idx, durations)
+        B = units.shape[0]
+        if B > 1 and B * x0.Tp * self._max_rate() > self.MAX_GEMM_ROWS:
+            # too many frames for one pass: the halves are generated on their own (each row is masked to its own length,
+            # so a row's samples do not depend on the rows it is batched with), with the durations already predicted
+            h = B // 2
+            parts = [self.resynthesize(units[r0:r1], lang_idx[r0:r1], spkr_idx[r0:r1], dur[r0:r1])[0]
+                     for r0, r1 in ((0, h), (h, B))]
+            wav = torch.zeros((B, 1, max(p.shape[-1] for p in parts)), dtype=torch.float32, device=self.device)
+            wav[:h, :, :parts[0].shape[-1]] = parts[0]
+            wav[h:, :, :parts[1].shape[-1]] = parts[1]
+            return wav, tot.to(torch.int64) * self.cfg.hop, dur
         return self._generate(x0, lens), tot.to(torch.int64) * self.cfg.hop, dur
+
+    # one sb_gemm call covers at most 65535 row tiles of 128 rows (the grid's y extent)
+    MAX_GEMM_ROWS = 65535 * 128
+
+    def _fused_stage(self, cout: int) -> bool:
+        """The stage's ResBlocks run as fused kernels (resblock.cu) rather than conv by conv on sb_gemm."""
+        c = self.cfg
+        return self.fused_resblocks and cout in (16, 32) and all(
+            len(dl) == 3 and rk % 2 == 1 and rk <= 11 and (rk - 1) // 2 * max(dl) <= 32
+            for rk, dl in zip(c.resblock_kernel_sizes, c.resblock_dilation_sizes))
+
+    def _max_rate(self) -> int:
+        """Rows per unit-rate frame of the longest sb_gemm of _generate: the last upsampling GEMM's input when the last
+        stage's ResBlocks are fused, else the full hop (its ResBlock convs run on sb_gemm at the output rate)."""
+        c = self.cfg
+        cout = c.upsample_initial_channel // 2 ** len(c.upsample_rates)
+        return c.hop // c.upsample_rates[-1] if self._fused_stage(cout) else c.hop
 
     def _expand(self, units, lang_idx, spkr_idx, durations=None):
         """Duration predictor + HardUpsampling of resynthesize() -> (x0 Seq (B, max T_b, model_in_dim) with rows past
@@ -1102,9 +1148,7 @@ class VocoderEngine:
             last_slope = 0.01 if i == nstage - 1 else 0.1  # F.leaky_relu default slope before conv_post (hifigan.py:192)
             L = None if lens is None else lens[i + 1]
             nxt_act = Seq(B, T, cout, PHn, Tp, lens=L, zero="edges")
-            fused = self.fused_resblocks and cout in (16, 32) and all(
-                len(dl) == 3 and rk % 2 == 1 and rk <= 11 and (rk - 1) // 2 * max(dl) <= 32
-                for rk, dl in zip(c.resblock_kernel_sizes, c.resblock_dilation_sizes))
+            fused = self._fused_stage(cout)
             # masked at the input rate: row b's T_b input frames give its u*T_b output frames
             up_raw = Seq(act.B, act.T, u * cout, act.PH, act.Tp, lens=act.lens, zero="edges")
             up_act = None if fused else Seq(act.B, act.T, u * cout, act.PH, act.Tp, lens=act.lens, zero="edges")

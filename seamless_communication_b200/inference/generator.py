@@ -10,7 +10,7 @@ from typing import Any, List, Optional, Tuple
 import torch
 from torch import Tensor
 
-from ..models.unity import UnitTokenizer, UnitYModel
+from ..models.unity import UnitTokenizer, UnitYModel, UnitYT2UModel
 from ..nn import PaddingMask
 from ..ops import Seq
 
@@ -30,6 +30,14 @@ def remove_consecutive_repeated_ngrams(sequence: List[int], min_size: int = 1, m
                 break
         start += 1
     return [tok for i, tok in enumerate(sequence) if i not in drop]
+
+
+def filter_unit_ngrams(units: Tensor) -> Tensor:
+    """`ngram_filtering` of the AR T2U's decoded units (generator.py:356-362): batch 1 only, as in the reference."""
+    if units.size(0) > 1:
+        raise NotImplementedError("unit ngram_filtering is not implemented for batch_size > 1.")
+    arr = remove_consecutive_repeated_ngrams(units[0].tolist())
+    return torch.tensor(arr).to(units).unsqueeze(0)
 
 
 @dataclass
@@ -59,6 +67,8 @@ class UnitYGenerator:
         model.eval()
         self.model = model
         self.text_opts = text_opts or SequenceGeneratorOptions()
+        # generator.py:205-210: the AR T2U's own default (speech sequences are much longer than text)
+        self.unit_opts = unit_opts or SequenceGeneratorOptions(soft_max_seq_len=(25, 50), hard_max_seq_len=5000)
         if model.text_decoder is None:
             raise ValueError("`UnitYGenerator` requires a text decoder, but the current UnitY model does not have one.")
         if self.text_opts.step_processor is not None:
@@ -75,6 +85,8 @@ class UnitYGenerator:
                 raise ValueError("`model` does not have a T2U sub-model when `unit_tokenizer` is not None.")
             self.unit_decoder = unit_tokenizer.create_decoder()
             self.unit_prefix_indices = unit_tokenizer.create_encoder(lang=target_lang).prefix_indices
+            if isinstance(model.t2u_model, UnitYT2UModel) and self.unit_opts.step_processor is not None:
+                raise NotImplementedError("step processors (MinTox banned sequences) are outside the S2ST hot path")
 
     @torch.inference_mode()
     def __call__(self, source_seqs: Tensor, source_padding_mask: Optional[PaddingMask], input_modality: str = "speech",
@@ -117,7 +129,34 @@ class UnitYGenerator:
         if dec is None:
             dec = eng.decode_full(text_seqs, text_lens, enc, enc_lens)
         assert self.model.t2u_model is not None and self.unit_decoder is not None
+        if isinstance(self.model.t2u_model, UnitYT2UModel):
+            return texts, self._generate_units_ar(dec, text_lens, ngram_filtering)
         units, unit_lens, aux = eng.t2u(dec, text_seqs, duration_factor)
         # engine.t2u already applied argmax -> pad mask -> UnitTokenDecoder (generator.py:346-353) on device
         self.last_unit_output = dict(unit_lens=unit_lens, text_seqs=text_seqs, dec_out=dec, **aux)
         return texts, units
+
+    def _generate_units_ar(self, dec: Seq, text_lens: Tensor, ngram_filtering: bool) -> Tensor:
+        """generator.py:316-362 for the AR T2U: T2U encoder over the decoder states (text padding mask), unit beam search
+        from the prefix [eos, lang] (echo_prompt=True: the hypotheses hold it), best hypothesis per row padded with the
+        pad symbol, UnitTokenDecoder.  `last_unit_output["unit_lens"]` holds each row's decoded length (its EOS, turned
+        into the pad symbol, included)."""
+        t2u = self.model.t2u_model
+        t2u_enc = self.model.engine.t2u_encode(dec)
+        o = self.unit_opts
+        hyps = t2u.beam_search(t2u_enc, text_lens, self.unit_prefix_indices.tolist(), beam=o.beam_size,
+                               soft_max=o.soft_max_seq_len, hard_max=o.hard_max_seq_len, len_penalty=o.len_penalty,
+                               unk_penalty=o.unk_penalty)
+        for h in hyps:
+            if not h:
+                raise RuntimeError("The sequence generator returned no hypothesis at index 0. Please file a bug report.")
+        seqs = [h[0][1] for h in hyps]
+        unit_seqs = torch.full((len(seqs), max(len(s) for s in seqs)), t2u.target_vocab_info.pad_idx, dtype=torch.int64)
+        for i, s in enumerate(seqs):
+            unit_seqs[i, :len(s)] = torch.tensor(s)
+        units = self.unit_decoder(unit_seqs)
+        if ngram_filtering:
+            units = filter_unit_ngrams(units)
+        self.last_unit_output = dict(hypotheses=hyps, t2u_enc=t2u_enc, dec_out=dec,
+                                     unit_lens=[units.size(1)] if ngram_filtering else [len(s) - 1 for s in seqs])
+        return units

@@ -6,12 +6,14 @@ from dataclasses import dataclass
 from enum import Enum, auto
 from typing import List, Optional, Tuple, Union, cast
 
+import threading
+
 import torch
 from torch import Tensor
 
 from .. import config as cfgmod
 from .. import ops
-from ..models.unity import UnitTokenizer, UnitYModel, load_unity_model
+from ..models.unity import UnitTokenizer, UnitYModel, UnitYT2UModel, load_unity_model
 from ..models.vocoder import Vocoder, load_vocoder_model
 from ..nn import PaddingMask, SequenceData, get_seqs_and_padding_mask
 from .generator import SequenceGeneratorOptions, UnitYGenerator
@@ -38,6 +40,8 @@ class BatchedSpeechOutput:
 
 
 class Translator:
+    _tls = threading.local()  # the calling thread's last generator (LanePool workers call predict concurrently)
+
     def __init__(self, model_name_or_card: Union[str, UnitYModel], vocoder_name_or_card: Union[str, Vocoder, None], device,
                  text_tokenizer=None, apply_mintox: bool = False, dtype=torch.float16,
                  input_modality: Optional[Modality] = None, output_modality: Optional[Modality] = None, **model_kw):
@@ -112,7 +116,7 @@ class Translator:
                        prosody_encoder_input=None) -> Tuple[List[str], Optional[Tensor]]:
         generator = UnitYGenerator(model, text_tokenizer, tgt_lang, unit_tokenizer if output_modality == Modality.SPEECH else None,
                                    text_opts=text_generation_opts, unit_opts=unit_generation_opts)
-        cls._last_generator = generator
+        cls._last_generator = cls._tls.generator = generator
         return generator(seqs, padding_mask, input_modality.value, output_modality.value,
                          ngram_filtering=unit_generation_ngram_filtering, duration_factor=duration_factor,
                          prosody_encoder_input=prosody_encoder_input)
@@ -139,8 +143,12 @@ class Translator:
                 prosody_encoder_input=None, src_text=None) -> Tuple[List[str], Optional[BatchedSpeechOutput]]:
         input_modality, output_modality = self.get_modalities_from_task_str(task_str)
         if output_modality == Modality.SPEECH and self.model.config.encoder_variant == "v1":
-            raise NotImplementedError(f"{task_str.upper()} on {self.model.config.name} needs its autoregressive T2U (the "
-                                      "v1 AR T2U model), which is not implemented; S2TT and ASR are")
+            if self.model.t2u_model is None:
+                raise NotImplementedError(f"{task_str.upper()} on {self.model.config.name} needs its autoregressive T2U (the "
+                                          "v1 AR T2U model), which this model was loaded without; S2TT and ASR run")
+            if input_modality == Modality.TEXT:
+                raise NotImplementedError(f"{task_str.upper()} on {self.model.config.name} needs text input (the NLLB text "
+                                          "encoder), which is not implemented; S2ST, S2TT and ASR are")
         if self.apply_mintox and not (src_lang is not None or src_text is not None):
             raise ValueError("`src_lang` must be specified when `apply_mintox` is `True` or you need to specify src_text.")
         if isinstance(input, dict):
@@ -173,6 +181,9 @@ class Translator:
             return texts, None
         assert units is not None and self.model.t2u_model is not None
         pad_idx = self.model.t2u_model.target_vocab_info.pad_idx
+        if isinstance(self.model.t2u_model, UnitYT2UModel):
+            return texts, self._speech_output_ar(units, self._tls.generator.last_unit_output["unit_lens"], tgt_lang, spkr,
+                                                 sample_rate)
         # translator.py:396-404 incl. the quirk that a genuine unit 1 is dropped like a pad (SURVEY a16)
         units_host = units.cpu()
         speech_units = [u[u != pad_idx].tolist() for u in units_host]
@@ -183,3 +194,26 @@ class Translator:
                 n = int(wav.size(-1) * len(speech_units[i]) / len(units[i]))
                 audio_wavs.append(wav[i, :, :n].unsqueeze(0))
         return texts, BatchedSpeechOutput(units=speech_units, audio_wavs=audio_wavs, sample_rate=sample_rate)
+
+    def _speech_output_ar(self, units: Tensor, unit_lens: List[int], tgt_lang: str, spkr: Optional[int],
+                          sample_rate: int) -> BatchedSpeechOutput:
+        """translator.py:386-428 for the AR T2U: the language token is dropped, `speech_units` loses every 1 (the pad
+        quirk), and the vocoder predicts durations.  Row b is what the reference returns for that row alone at batch 1
+        (it cannot vocode a batch whose rows expand to different lengths): the vocoder input is the row's own units, its
+        EOS-turned-1 included, without padding, and the waveform is trimmed to
+        int(hop * T_b * len(speech_units_b) / len(units_b)) of its own hop * T_b samples.  Rows with the same number of
+        units are vocoded together; each row of such a batch equals the row vocoded alone."""
+        pad_idx = self.model.t2u_model.target_vocab_info.pad_idx
+        rows = [units[i, 1:n].cpu() for i, n in enumerate(unit_lens)]
+        speech_units = [r[r != pad_idx].tolist() for r in rows]
+        audio_wavs: List[Tensor] = []
+        if self.vocoder is not None:
+            wavs: List[Optional[Tensor]] = [None] * len(rows)
+            for n in sorted({r.numel() for r in rows}):
+                idx = [i for i, r in enumerate(rows) if r.numel() == n]
+                wav = self.vocoder(torch.stack([rows[i] for i in idx]).to(self.device), tgt_lang, spkr, dur_prediction=True)
+                for j, i in enumerate(idx):
+                    keep = int(int(self.vocoder.last_wav_lens[j]) * len(speech_units[i]) / n)
+                    wavs[i] = wav[j, :, :keep].unsqueeze(0)
+            audio_wavs = cast(List[Tensor], wavs)
+        return BatchedSpeechOutput(units=speech_units, audio_wavs=audio_wavs, sample_rate=sample_rate)

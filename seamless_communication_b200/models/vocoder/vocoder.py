@@ -1,6 +1,7 @@
 """Vocoder facade (reference models/vocoder/vocoder.py:15-49) over the CUDA Code-HiFiGAN engine."""
 from __future__ import annotations
 
+import threading
 from typing import Any, Dict, List, Optional, Union
 
 import torch
@@ -15,7 +16,12 @@ class Vocoder:
     def __init__(self, engine: VocoderEngine, lang_spkr_idx_map: Dict[str, Any]):
         self.code_generator = engine
         self.lang_spkr_idx_map = lang_spkr_idx_map
-        self.last_wav_lens: Optional[Tensor] = None  # (N,) int64 samples per row of the last dur_prediction=True call
+        self._tls = threading.local()  # LanePool workers vocode concurrently: each thread sees its own last call
+
+    @property
+    def last_wav_lens(self) -> Optional[Tensor]:
+        """(N,) int64 samples per row of this thread's last dur_prediction=True call."""
+        return getattr(self._tls, "wav_lens", None)
 
     def eval(self):
         return self
@@ -45,7 +51,7 @@ class Vocoder:
             if not getattr(self.code_generator, "has_dur_predictor", False):
                 raise NotImplementedError("dur_prediction=True needs a vocoder loaded with its duration predictor "
                                           "(code_generator.dur_predictor.*)")
-            wav, self.last_wav_lens, _ = self.code_generator.resynthesize(units.reshape(n, -1), lang_ids, spkr_ids)
+            wav, self._tls.wav_lens, _ = self.code_generator.resynthesize(units.reshape(n, -1), lang_ids, spkr_ids)
             return wav
         return self.code_generator(units.reshape(n, -1), lang_ids, spkr_ids)
 
@@ -56,7 +62,8 @@ def load_vocoder_model(name_or_arch: str, device="cuda", dtype=torch.float16, st
                        synthetic: bool = False) -> Vocoder:
     """Weights: `state_dict` ("code_generator.*" keys), or `checkpoint` (path / mapping, {"generator": ...} of the original
     release or {"model": ...}; models/checkpoint.py), or `synthetic=True` for seeded random-init weights.  Without any of
-    them a RuntimeError is raised instead of silently vocoding with random weights."""
+    them a RuntimeError is raised instead of silently vocoding with random weights.  The language / speaker table is the
+    card's: `vocoder_36langs` (seamlessM4T_large) has its own speaker ids, every other name gets vocoder_v2's."""
     arch = cfgmod.VOCODER_CARDS.get(name_or_arch, name_or_arch)
     if arch not in cfgmod.VOCODER_ARCHS:
         raise ValueError(f"unknown vocoder card / architecture '{name_or_arch}'")
@@ -68,5 +75,6 @@ def load_vocoder_model(name_or_arch: str, device="cuda", dtype=torch.float16, st
     if state_dict is None:
         if not synthetic:
             raise RuntimeError(f"no weights for vocoder '{name_or_arch}': pass state_dict=..., checkpoint=... or synthetic=True")
-        state_dict = synthetic_mod.make_vocoder_state_dict(cfg, seed=seed)
-    return Vocoder(VocoderEngine(cfg, state_dict, device=device), cfgmod.vocoder_lang_spkr_idx_map())
+        # vocoder_36langs serves seamlessM4T_large's deduplicated units: its checkpoint carries the duration predictor
+        state_dict = synthetic_mod.make_vocoder_state_dict(cfg, seed=seed, dur_predictor=name_or_arch == "vocoder_36langs")
+    return Vocoder(VocoderEngine(cfg, state_dict, device=device), cfgmod.vocoder_lang_spkr_idx_map(name_or_arch))

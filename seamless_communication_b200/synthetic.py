@@ -69,19 +69,23 @@ class _Init:
 
 
 def make_unity_state_dict(cfg: UnitYConfig, seed: int = 0, logit_scale: float = 4.0,
-                          with_t2u: bool = True, dur_gain: float = 0.02, dur_bias: float = 0.0,
+                          with_t2u: Optional[bool] = None, dur_gain: float = 0.02, dur_bias: float = 0.0,
                           embed_scale: float = 0.25, dec_gain: float = 1.0) -> Dict[str, torch.Tensor]:
     """Random-init UnitY2 parameters under the reference's state_dict names (SURVEY 8b).
 
     With cfg.encoder_variant == "v1" the Conformer layers carry the w2v-BERT v1 parameters instead of the Shaw table and
     the conv-module LayerNorm: `self_attn.sdpa.r_proj` (no bias), `u_bias` / `v_bias` (H, 64) and
-    `conv.batch_norm.{weight,bias,running_mean,running_var}` with non-trivial running statistics; no T2U is drawn.
+    `conv.batch_norm.{weight,bias,running_mean,running_var}` with non-trivial running statistics.  Its T2U is the
+    autoregressive one (t2u_builder.py:311-427): `t2u_model.encoder.*`, `t2u_model.decoder_frontend.embed`,
+    `t2u_model.decoder.layers.*` with `encoder_decoder_attn`, `t2u_model.decoder.layer_norm` and `t2u_model.final_proj`
+    tied to the embedding.  It is drawn after every other tensor, and only with with_t2u=True: the default (None) draws
+    the T2U of v2 architectures only, so the v1 text-only state dicts stay what they were.
     The v2 draws, and so every v2 state dict, are unchanged."""
     I = _Init(seed)
     M = cfg.model_dim
     v1 = cfg.encoder_variant == "v1"
-    if v1:
-        with_t2u = False
+    if with_t2u is None:
+        with_t2u = not v1
     fd = cfg.fbank_channels * cfg.fbank_stride
     I.ln("speech_encoder_frontend.post_extract_layer_norm", fd)
     I.linear("speech_encoder_frontend.model_dim_proj", M, fd)
@@ -147,7 +151,9 @@ def make_unity_state_dict(cfg: UnitYConfig, seed: int = 0, logit_scale: float = 
     I.sd["text_decoder.layer_norm.weight"] = _round_fp16(
         I.sd["text_decoder.layer_norm.weight"] * (logit_scale / embed_scale))
 
-    if with_t2u:
+    if with_t2u and v1:
+        _draw_ar_t2u(I, cfg, logit_scale, embed_scale)
+    elif with_t2u:
         for i in range(cfg.t2u_enc_layers):
             p = f"t2u_model.encoder.layers.{i}"
             I.ln(f"{p}.self_attn_layer_norm", M)
@@ -186,6 +192,38 @@ def make_unity_state_dict(cfg: UnitYConfig, seed: int = 0, logit_scale: float = 
         I.sd["t2u_model.decoder.layer_norm.weight"] = _round_fp16(
             I.sd["t2u_model.decoder.layer_norm.weight"] * (logit_scale / embed_scale))
     return I.sd
+
+
+def _draw_ar_t2u(I: _Init, cfg: UnitYConfig, logit_scale: float, embed_scale: float) -> None:
+    """The autoregressive T2U of seamlessM4T_large (t2u_builder.py:311-427), scaled like the text decoder: a small tied
+    unit embedding and a final LayerNorm gain that peaks the logits."""
+    M = cfg.model_dim
+    for i in range(cfg.t2u_enc_layers):
+        p = f"t2u_model.encoder.layers.{i}"
+        I.ln(f"{p}.self_attn_layer_norm", M)
+        I.mha(f"{p}.self_attn", M)
+        I.ln(f"{p}.ffn_layer_norm", M)
+        I.linear(f"{p}.ffn.inner_proj", cfg.t2u_ffn_dim, M)
+        I.linear(f"{p}.ffn.output_proj", M, cfg.t2u_ffn_dim)
+    I.ln("t2u_model.encoder.layer_norm", M)
+    uemb = I.normal("t2u_model.decoder_frontend.embed.weight", (cfg.unit_vocab, M), embed_scale * M ** -0.5)
+    # control symbols and the language symbols score 0: the search only emits units in [4, num_units + 4), which the
+    # vocoder's table can hold, and EOS only at the forced last step
+    uemb[:4].zero_()
+    uemb[cfg.num_units + 4:].zero_()
+    I.sd["t2u_model.final_proj.weight"] = uemb
+    for i in range(cfg.t2u_dec_layers):
+        p = f"t2u_model.decoder.layers.{i}"
+        I.ln(f"{p}.self_attn_layer_norm", M)
+        I.mha(f"{p}.self_attn", M)
+        I.ln(f"{p}.encoder_decoder_attn_layer_norm", M)
+        I.mha(f"{p}.encoder_decoder_attn", M)
+        I.ln(f"{p}.ffn_layer_norm", M)
+        I.linear(f"{p}.ffn.inner_proj", cfg.t2u_ffn_dim, M)
+        I.linear(f"{p}.ffn.output_proj", M, cfg.t2u_ffn_dim)
+    I.ln("t2u_model.decoder.layer_norm", M)
+    I.sd["t2u_model.decoder.layer_norm.weight"] = _round_fp16(
+        I.sd["t2u_model.decoder.layer_norm.weight"] * (logit_scale / embed_scale))
 
 
 def make_vocoder_state_dict(cfg: VocoderConfig, seed: int = 1, dur_predictor: bool = False, dur_gain: float = 0.3,
