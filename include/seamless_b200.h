@@ -312,8 +312,11 @@ int sb_text_to_chars(const int32_t* text_seqs, int32_t L, int32_t batch, const u
                      int32_t unk_idx, int32_t eos_idx, int32_t* char_lens, int32_t* char_seqs, int32_t max_c,
                      int32_t* char_seq_lens, sb_stream_t stream);
 /* HardUpsampling + additive terms: y[b][u] = x[b][src(u)] + alpha*pos[u] + (emb ? emb[ids[b][u]]*emb_scale : 0)
- * for u < sum(dur[b]); zeros beyond... (+ pos/emb exactly as the reference adds them to padded rows too).
- *   x in sequence layout (x_rows,x_halo), y in sequence layout (y_rows,y_halo), U = y logical length. */
+ * for u < sum(dur[b]), and exact zeros for sum(dur[b]) <= u < U: pos / emb are not added there, so those rows are the
+ * zero padding the next conv reads (the reference adds them to padded rows too; every consumer masks those rows).
+ *   x in sequence layout (x_rows,x_halo), y in sequence layout (y_rows,y_halo), U = y logical length; pos_table fp32
+ *   [U][dim] or NULL, alpha a device fp32 scalar or NULL (0), emb fp16 or NULL; out_lens[b] = sum(dur[b]) if given.
+ *   SB_ENOSUP for S > 10240 (the prefix sums of the durations live in 40 KB of shared memory). */
 int sb_upsample_add(const void* x, int32_t x_rows, int32_t x_halo, int32_t S, const int32_t* dur, void* y,
                     int32_t y_rows, int32_t y_halo, int32_t U, int32_t batch, int32_t dim, const void* pos_table,
                     const float* alpha, const void* emb, const int32_t* ids, int32_t ids_ld, float emb_scale,

@@ -138,12 +138,13 @@ __global__ void durations_kernel(const elem_t* __restrict__ hidden, int rows_ld,
   }
   acc = warp_sum(acc) + bias;
   if (lane == 0) {
-
     const float logd = acc;
+    // float -> s64 saturates; durations past INT32_MAX are clamped to it rather than wrapped to their low 32 bits, so
+    // that the callers' length checks see them as too long
     long long d = (long long)rintf((expf(logd) - 1.f) * factor);
     if (d < 1) d = 1;
     if (lens != nullptr && s >= lens[b]) d = 0;
-    dur[idx] = (int)d;
+    dur[idx] = (int)min(d, (long long)INT_MAX);
   }
 }
 

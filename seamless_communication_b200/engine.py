@@ -938,6 +938,26 @@ class UnitYEngine:
         return units.to(torch.int64), unit_lens, aux
 
 
+def conv_transpose_taps(cw: torch.Tensor, u: int, k: int) -> torch.Tensor:
+    """ConvTranspose1d(stride u, kernel k, padding (k - u) // 2) weights (cin, cout, k) -> (u * cout, 3 * cin) weights
+    of a zero-padded 3-tap conv at the input rate whose u * cout outputs per input frame are the u output frames of
+    that frame, phase-major: output frame q * u + p = sum_t w[p, :, t, :] . x[q + t - 1], tap j = p + pad - (t - 1) * u
+    of the transposed conv.  Only k - u even (u * T output frames) with every tap j in [0, k) reached by some (p, t),
+    i.e. u <= k <= 3 u, has this form; anything else raises ValueError instead of dropping taps."""
+    cin, cout = cw.shape[0], cw.shape[1]
+    if cw.shape[2] != k or u < 1 or (k - u) % 2 or not u <= k <= 3 * u:
+        raise ValueError(f"ConvTranspose1d(stride {u}, kernel {k}) with weights {tuple(cw.shape)} is not a 3-tap conv "
+                         f"over the input frames (needs k - u even and u <= k <= 3u)")
+    pad = (k - u) // 2
+    wt = torch.zeros(u, cout, 3, cin, dtype=cw.dtype)
+    for p in range(u):
+        for t in range(3):
+            j = p + pad - (t - 1) * u
+            if 0 <= j < k:
+                wt[p, :, t, :] = cw[:, :, j].t()
+    return wt.reshape(u * cout, 3 * cin)
+
+
 class VocoderEngine:
     """Code-HiFiGAN (models/vocoder/{vocoder,codehifigan,hifigan}.py) on sb_gemm."""
 
@@ -977,15 +997,7 @@ class VocoderEngine:
         conv("conv_pre")
         ch = c.upsample_initial_channel
         for i, (u, k) in enumerate(zip(c.upsample_rates, c.upsample_kernel_sizes)):
-            cw = folded(f"ups.{i}")  # ConvTranspose1d weight (in, out, k)
-            cin, cout, pad = cw.shape[0], cw.shape[1], (k - u) // 2
-            wt = torch.zeros(u, cout, 3, cin)
-            for p in range(u):
-                for t in range(3):
-                    j = p + pad - (t - 1) * u
-                    if 0 <= j < k:
-                        wt[p, :, t, :] = cw[:, :, j].t()
-            w[f"ups.{i}.w"] = wt.reshape(u * cout, 3 * cin).to(dev, F16).contiguous()
+            w[f"ups.{i}.w"] = conv_transpose_taps(folded(f"ups.{i}"), u, k).to(dev, F16).contiguous()
             w[f"ups.{i}.b"] = sd[P + f"ups.{i}.bias"].float().repeat(u).to(dev).contiguous()
             for j in range(len(c.resblock_kernel_sizes)):
                 rb = i * len(c.resblock_kernel_sizes) + j
