@@ -211,6 +211,26 @@ int sb_logits_topk_tiles(const float* logits, int64_t ld, const float* tile_stat
                          int32_t eos_idx, int32_t unk_idx, float unk_penalty, int32_t K, float* cand_val, int32_t* cand_idx,
                          float* eos_lprob, sb_stream_t stream);
 
+/* Banned sequences (fairseq2 BannedSequenceProcessor, the MinTox re-decode) at one selecting step.  `table` is a device
+ * buffer: [0] the number of sequences (<= cap), [1 .. cap] their lengths (1 .. width), then cap rows of `width` tokens,
+ * each sequence right-aligned in its row.  Row r of seqs [rows][seq_ld] holds its hypothesis up to *step_ptr; a sequence
+ * s of length n bans s[n-1] when n == 1 or when seqs[r][step-n+2 .. step] == s[0 .. n-2].  Writes ban_n[r] and the banned
+ * ids of row r to ban_ids[r*cap ..] (unordered, duplicates possible, at most cap). */
+int sb_ban_step(const int32_t* seqs, int32_t seq_ld, const int32_t* step_ptr, int32_t rows, const int32_t* table, int32_t cap,
+                int32_t width, int32_t* ban_ids, int32_t* ban_n, sb_stream_t stream);
+
+/* sb_logits_topk / sb_logits_topk_tiles with row r's ids ban_ids[r*ban_ld .. + ban_n[r]] banned: a banned id is never a
+ * candidate, and eos_lprob is -inf when eos_idx is banned.  The log-sum-exp still runs over the whole row, so every other
+ * lprob is the one the unbanned entry returns, bit for bit.  Any number of bans per row: the vocabulary bitmap takes
+ * (vocab + 31) / 32 words of shared memory. */
+int sb_logits_topk_ban(const float* logits, int64_t ld, int32_t rows, int32_t vocab, int32_t pad_idx, int32_t eos_idx,
+                       int32_t unk_idx, float unk_penalty, int32_t K, float* cand_val, int32_t* cand_idx, float* eos_lprob,
+                       const int32_t* ban_ids, const int32_t* ban_n, int32_t ban_ld, sb_stream_t stream);
+int sb_logits_topk_tiles_ban(const float* logits, int64_t ld, const float* tile_stats, int32_t rows, int32_t vocab,
+                             int32_t pad_idx, int32_t eos_idx, int32_t unk_idx, float unk_penalty, int32_t K, float* cand_val,
+                             int32_t* cand_idx, float* eos_lprob, const int32_t* ban_ids, const int32_t* ban_n, int32_t ban_ld,
+                             sb_stream_t stream);
+
 /* one beam-search step for every sentence (BeamSearchSeq2SeqGenerator step, mirrored fairseq2.cpp:1463-1594).
  * State (all device, int32/fp32):
  *   seqs [B*beam][max_len], scores [B*beam][max_len], anc [B*beam][max_len],

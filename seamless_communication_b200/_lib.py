@@ -108,6 +108,9 @@ PROTOTYPES = {
     "sb_logits_topk": [c_p, i64, i32, i32, i32, i32, i32, f32, i32, c_p, c_p, c_p, c_p],
     "sb_logits_topk_tiles": [c_p, i64, c_p, i32, i32, i32, i32, i32, f32, i32, c_p, c_p, c_p, c_p],
     "sb_beam_step": [C.POINTER(BeamDesc), c_p],
+    "sb_ban_step": [c_p, i32, c_p, i32, c_p, i32, i32, c_p, c_p, c_p],
+    "sb_logits_topk_ban": [c_p, i64, i32, i32, i32, i32, i32, f32, i32, c_p, c_p, c_p, c_p, c_p, i32, c_p],
+    "sb_logits_topk_tiles_ban": [c_p, i64, c_p, i32, i32, i32, i32, i32, f32, i32, c_p, c_p, c_p, c_p, c_p, i32, c_p],
     "sb_kv_heads_major": [c_p, i64, i32, i32, i32, c_p, c_p, c_p],
     "sb_decoder_plan_query": [i32, i32, i32, i32, i32, i32, C.POINTER(DecoderPlanInfo)],
     "sb_decoder_plan_init": [C.POINTER(DecoderPlanDesc), C.POINTER(DecoderLaunch)],

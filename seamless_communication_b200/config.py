@@ -238,3 +238,10 @@ VOCODER_ARCHS = {"base": base_vocoder, "tiny": tiny_vocoder}
 MODEL_CARDS = {"seamlessM4T_v2_large": "base_v2", "seamlessM4T_v2_tiny": "tiny_v2", "seamlessM4T_v2_small": "small_v2",
                "seamlessM4T_large": "base"}
 VOCODER_CARDS = {"vocoder_v2": "base", "vocoder_v2_tiny": "tiny", "vocoder_36langs": "base"}
+
+# cards/mintox.yaml (the ETOX word lists of MinTox, toxicity/etox_bad_word_checker.py): word files named after one of
+# these language variants keep the full name, every other file its first three letters; the languages in SP_LANGS are
+# matched by SentencePiece token subsequence instead of by whole words (tests/golden/mintox_card.json pins both)
+MINTOX_ETOX_LANG_VARIANTS = ("kas_Arab", "kas_Deva", "knc_Arab", "knc_Latn", "min_Arab", "min_Latn", "zho_Hans", "zho_Hant")
+MINTOX_SP_LANGS = ("asm", "ben", "cmn", "guj", "mya", "hin", "gom", "ibo", "jpn", "kan", "khm", "kor", "lao", "mai", "mal",
+                   "mar", "mni", "npi", "oan", "ory", "pan", "rwr", "sat", "tam", "tel", "tha", "wuu", "yue")

@@ -487,10 +487,37 @@ __device__ __forceinline__ float tk_cand(float x, int i, int pad_idx, int unk_id
   return x;
 }
 
+// Banned sequences (sb_ban_step writes each row's banned token ids): the row's list becomes a vocabulary bitmap in
+// dynamic shared memory (32 KB at 256 102 tokens), so that a test costs one shared load whatever the list's length.
+__device__ __forceinline__ bool tk_banned(const unsigned* bits, int i) { return (bits[i >> 5] >> (i & 31)) & 1u; }
+
+__device__ __forceinline__ void tk_load_bans(unsigned* bits, int vocab, const int* __restrict__ ids, int n) {
+  for (int i = threadIdx.x; i < (vocab + 31) / 32; i += blockDim.x) bits[i] = 0u;
+  __syncthreads();
+  for (int j = threadIdx.x; j < n; j += blockDim.x) {
+    const int id = ids[j];
+    if (id >= 0 && id < vocab) atomicOr(bits + (id >> 5), 1u << (id & 31));
+  }
+  __syncthreads();
+}
+
+// a banned token is not a candidate; the normaliser still includes it (bans apply after log_softmax)
+template <bool BAN>
+__device__ __forceinline__ float tk_cand_b(float x, int i, int pad_idx, int unk_idx, float unk_penalty, const unsigned* bits) {
+  if constexpr (BAN) {
+    if (tk_banned(bits, i)) return -INFINITY;
+  }
+  return tk_cand(x, i, pad_idx, unk_idx, unk_penalty);
+}
+
+// BAN: row r's banned ids are ban_ids[r * ban_ld .. + ban_n[r]] (dynamic shared memory: the vocabulary bitmap)
+template <bool BAN>
 __global__ void __launch_bounds__(TK_THREADS) logits_topk_kernel(const float* __restrict__ logits, long long ld, int vocab,
                                                                  int pad_idx, int eos_idx, int unk_idx, float unk_penalty, int K,
                                                                  float* __restrict__ cand_val, int* __restrict__ cand_idx,
-                                                                 float* __restrict__ eos_lprob) {
+                                                                 float* __restrict__ eos_lprob, const int* __restrict__ ban_ids,
+                                                                 const int* __restrict__ ban_n, int ban_ld) {
+  extern __shared__ unsigned tk_bits[];
   pdl_sync();
   const int r = blockIdx.x;
   const float* row = logits + (long long)r * ld;
@@ -501,6 +528,7 @@ __global__ void __launch_bounds__(TK_THREADS) logits_topk_kernel(const float* __
   __shared__ int s_count;
   __shared__ float s_cv[TK_CAP];
   __shared__ int s_ci[TK_CAP];
+  if constexpr (BAN) tk_load_bans(tk_bits, vocab, ban_ids + (long long)r * ban_ld, min(ban_n[r], ban_ld));
   const int nvec = vocab >> 2;
   // ---- pass 1
   float mx = -INFINITY, sum = 0.f, best = -INFINITY;
@@ -512,14 +540,14 @@ __global__ void __launch_bounds__(TK_THREADS) logits_topk_kernel(const float* __
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       sum += __expf(xs[e] - mx);
-      best = fmaxf(best, tk_cand(xs[e], 4 * i + e, pad_idx, unk_idx, unk_penalty));
+      best = fmaxf(best, tk_cand_b<BAN>(xs[e], 4 * i + e, pad_idx, unk_idx, unk_penalty, tk_bits));
     }
   }
   for (int i = 4 * nvec + threadIdx.x; i < vocab; i += TK_THREADS) {
     const float x = row[i];
     if (x > mx) { sum *= __expf(mx - x); mx = x; }
     sum += __expf(x - mx);
-    best = fmaxf(best, tk_cand(x, i, pad_idx, unk_idx, unk_penalty));
+    best = fmaxf(best, tk_cand_b<BAN>(x, i, pad_idx, unk_idx, unk_penalty, tk_bits));
   }
   s_best[threadIdx.x] = best;
   {
@@ -536,7 +564,7 @@ __global__ void __launch_bounds__(TK_THREADS) logits_topk_kernel(const float* __
     for (int i = 0; i < TK_THREADS / 32; ++i) S += s_s[i] * __expf(s_m[i] - M);
     if (lane == 0) {
       s_lse = M + logf(S);
-      eos_lprob[r] = row[eos_idx] - (M + logf(S));
+      eos_lprob[r] = (BAN && tk_banned(tk_bits, eos_idx)) ? -INFINITY : row[eos_idx] - (M + logf(S));
     }
     // K-th largest of the 512 per-thread bests: each lane owns 16 of them
     float loc[TK_THREADS / 32];
@@ -566,7 +594,7 @@ __global__ void __launch_bounds__(TK_THREADS) logits_topk_kernel(const float* __
     const float xs[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
-      const float cv = tk_cand(xs[e], 4 * i + e, pad_idx, unk_idx, unk_penalty);
+      const float cv = tk_cand_b<BAN>(xs[e], 4 * i + e, pad_idx, unk_idx, unk_penalty, tk_bits);
       if (cv >= tau && cv > -INFINITY) {
         const int slot = atomicAdd(&s_count, 1);
         if (slot < TK_CAP) { s_cv[slot] = cv; s_ci[slot] = 4 * i + e; }
@@ -574,7 +602,7 @@ __global__ void __launch_bounds__(TK_THREADS) logits_topk_kernel(const float* __
     }
   }
   for (int i = 4 * nvec + threadIdx.x; i < vocab; i += TK_THREADS) {
-    const float cv = tk_cand(row[i], i, pad_idx, unk_idx, unk_penalty);
+    const float cv = tk_cand_b<BAN>(row[i], i, pad_idx, unk_idx, unk_penalty, tk_bits);
     if (cv >= tau && cv > -INFINITY) {
       const int slot = atomicAdd(&s_count, 1);
       if (slot < TK_CAP) { s_cv[slot] = cv; s_ci[slot] = i; }
@@ -613,15 +641,20 @@ __global__ void __launch_bounds__(TK_THREADS) logits_topk_kernel(const float* __
 //      candidate and the UNK penalty can push one more below);
 //   3. only the tiles whose maximum reaches tau are read back (one warp per tile, 512 B) and their elements >= tau collected;
 //   4. the same (value desc, index asc) extraction as logits_topk_kernel.
+// BAN: a tile whose maximum is a banned token ("tainted") takes no part in step 2, so tau is the (K+2)-th largest maximum
+// of the untainted tiles, each of which is reached by a token that is not banned: the bound holds whatever the number of
+// bans, and the candidate list does not grow with it.  Step 3 still reads tainted tiles and skips banned tokens.
 constexpr int TKT_THREADS = 256;
 constexpr int TKT_TILE = 128;
 
+template <bool BAN>
 __global__ void __launch_bounds__(TKT_THREADS) logits_topk_tiles_kernel(const float* __restrict__ logits, long long ld,
                                                                         const float2* __restrict__ stats, int rows, int vocab,
                                                                         int pad_idx, int eos_idx, int unk_idx, float unk_penalty, int K,
                                                                         float* __restrict__ cand_val, int* __restrict__ cand_idx,
-                                                                        float* __restrict__ eos_lprob) {
-  extern __shared__ float tk_sm[];  // tile maxima [n_tiles]
+                                                                        float* __restrict__ eos_lprob, const int* __restrict__ ban_ids,
+                                                                        const int* __restrict__ ban_n, int ban_ld) {
+  extern __shared__ float tk_sm[];  // tile maxima [n_tiles], live copy [n_tiles], BAN: vocabulary bitmap
   pdl_sync();
   const int r = blockIdx.x;
   const float* row = logits + (long long)r * ld;
@@ -633,6 +666,13 @@ __global__ void __launch_bounds__(TKT_THREADS) logits_topk_tiles_kernel(const fl
   __shared__ int s_count;
   __shared__ float s_cv[TK_CAP];
   __shared__ int s_ci[TK_CAP];
+  unsigned* bits = reinterpret_cast<unsigned*>(tk_sm + 2 * n_tiles);
+  const int* bans = ban_ids + (long long)r * ban_ld;
+  int n_ban = 0;
+  if constexpr (BAN) {
+    n_ban = min(ban_n[r], ban_ld);
+    tk_load_bans(bits, vocab, bans, n_ban);
+  }
   // ---- 1. row log-sum-exp
   float mx = -INFINITY;
   for (int i = threadIdx.x; i < n_tiles; i += TKT_THREADS) {
@@ -659,7 +699,7 @@ __global__ void __launch_bounds__(TKT_THREADS) logits_topk_tiles_kernel(const fl
     float S = 0.f;
     for (int i = 0; i < nwarp; ++i) S += s_red[i];
     s_lse = M + logf(S);
-    eos_lprob[r] = row[eos_idx] - (M + logf(S));
+    eos_lprob[r] = (BAN && tk_banned(bits, eos_idx)) ? -INFINITY : row[eos_idx] - (M + logf(S));
   }
   __syncthreads();
   // ---- 2. tau = (K+2)-th largest tile maximum (block-wide arg-max, K+2 rounds; the found tile is marked by negating into
@@ -668,6 +708,13 @@ __global__ void __launch_bounds__(TKT_THREADS) logits_topk_tiles_kernel(const fl
   float* live = tk_sm + n_tiles;
   for (int i = threadIdx.x; i < n_tiles; i += TKT_THREADS) live[i] = tk_sm[i];
   __syncthreads();
+  if constexpr (BAN) {
+    for (int j = threadIdx.x; j < n_ban; j += TKT_THREADS) {
+      const int id = bans[j];
+      if (id >= 0 && id < vocab && row[id] >= tk_sm[id / TKT_TILE]) live[id / TKT_TILE] = -INFINITY;
+    }
+    __syncthreads();
+  }
   const int rounds = min(K + 2, n_tiles);
   float tau = -INFINITY;
   for (int round = 0; round < rounds; ++round) {
@@ -711,7 +758,7 @@ __global__ void __launch_bounds__(TKT_THREADS) logits_topk_tiles_kernel(const fl
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       if (i0 + e >= vocab) continue;
-      const float cv = tk_cand(xs[e], i0 + e, pad_idx, unk_idx, unk_penalty);
+      const float cv = tk_cand_b<BAN>(xs[e], i0 + e, pad_idx, unk_idx, unk_penalty, bits);
       if (cv >= tau && cv > -INFINITY) {
         const int slot = atomicAdd(&s_count, 1);
         if (slot < TK_CAP) { s_cv[slot] = cv; s_ci[slot] = i0 + e; }
@@ -847,6 +894,35 @@ __global__ void __launch_bounds__(128) beam_step_kernel(const sb_beam_t p) {
   }
 }
 
+// Banned sequences at one selecting step (fairseq2 BannedSequenceProcessor): row r bans the last token of every table
+// sequence s of length n whose first n-1 tokens end the row, i.e. equal seqs[r][step-n+2 .. step] (n = 1: always).  The
+// rows are read after sb_beam_step reordered them, so they are the hypotheses the next top-K scores.  The table lives in
+// device memory ([0] count, [1 .. cap] lengths, then cap rows of `width` tokens, right-aligned), so one captured step
+// serves every table up to its capacity.  Output: ban_ids [rows][cap] (unordered, duplicates possible), ban_n [rows].
+__global__ void __launch_bounds__(256) ban_step_kernel(const int* __restrict__ seqs, int seq_ld, const int* __restrict__ step_ptr,
+                                                       const int* __restrict__ table, int cap, int width,
+                                                       int* __restrict__ ban_ids, int* __restrict__ ban_n) {
+  __shared__ int s_n;
+  pdl_sync();
+  const int r = blockIdx.x;
+  const int step = *step_ptr;
+  const int count = min(table[0], cap);
+  const int* lens = table + 1;
+  const int* toks = table + 1 + cap;
+  const int* row = seqs + (long long)r * seq_ld;
+  if (threadIdx.x == 0) s_n = 0;
+  __syncthreads();
+  for (int j = threadIdx.x; j < count; j += blockDim.x) {
+    const int n = lens[j];
+    const int* s = toks + (long long)j * width + width - n;
+    bool hit = n >= 1 && n <= width && n - 1 <= step + 1;  // a row of step+1 tokens cannot end in a longer prefix
+    for (int i = 0; hit && i < n - 1; ++i) hit = row[step + 2 - n + i] == s[i];
+    if (hit) ban_ids[(long long)r * cap + atomicAdd(&s_n, 1)] = s[n - 1];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) ban_n[r] = s_n;
+}
+
 // hist[step][...] = h: keeps the final-LayerNorm decoder state of every search step so that the states of the winning
 // hypothesis can be gathered afterwards instead of re-running the decoder teacher-forced (inference/generator.py:294-299)
 __global__ void store_step_kernel(const uint4* __restrict__ h, uint4* __restrict__ hist, const int* __restrict__ step_ptr, long long n16) {
@@ -961,9 +1037,27 @@ extern "C" int sb_logits_topk(const float* logits, int64_t ld, int32_t rows, int
   using namespace sb;
   SB_REQUIRE(logits && cand_val && cand_idx && eos_lprob && rows > 0 && vocab > 0, SB_EINVAL, "sb_logits_topk: bad args");
   SB_REQUIRE(K > 0 && K <= TK_MAX, SB_ENOSUP, "sb_logits_topk: K=%d unsupported (<= %d)", K, TK_MAX);
-  SB_CUDA_OK(launch_k(logits_topk_kernel, dim3(rows), dim3(TK_THREADS), 0, (cudaStream_t)stream, logits, (long long)ld,
+  SB_CUDA_OK(launch_k(logits_topk_kernel<false>, dim3(rows), dim3(TK_THREADS), 0, (cudaStream_t)stream, logits, (long long)ld,
                        (int)vocab, (int)pad_idx, (int)eos_idx, (int)unk_idx, unk_penalty, (int)K, cand_val, (int*)cand_idx,
-                       eos_lprob));
+                       eos_lprob, (const int*)nullptr, (const int*)nullptr, 0));
+  count_launch();
+  return SB_OK;
+}
+
+extern "C" int sb_logits_topk_ban(const float* logits, int64_t ld, int32_t rows, int32_t vocab, int32_t pad_idx, int32_t eos_idx,
+                                  int32_t unk_idx, float unk_penalty, int32_t K, float* cand_val, int32_t* cand_idx,
+                                  float* eos_lprob, const int32_t* ban_ids, const int32_t* ban_n, int32_t ban_ld,
+                                  sb_stream_t stream) {
+  using namespace sb;
+  SB_REQUIRE(logits && cand_val && cand_idx && eos_lprob && ban_ids && ban_n && rows > 0 && vocab > 0 && ban_ld > 0, SB_EINVAL,
+             "sb_logits_topk_ban: bad args");
+  SB_REQUIRE(K > 0 && K <= TK_MAX, SB_ENOSUP, "sb_logits_topk_ban: K=%d unsupported (<= %d)", K, TK_MAX);
+  const size_t smem = (size_t)(vocab + 31) / 32 * sizeof(unsigned);
+  SB_REQUIRE(smem <= 160 * 1024, SB_ENOSUP, "sb_logits_topk_ban: vocabulary of %d too large", vocab);
+  SB_CUDA_OK(allow_dynamic_smem(logits_topk_kernel<true>, smem));
+  SB_CUDA_OK(launch_k(logits_topk_kernel<true>, dim3(rows), dim3(TK_THREADS), smem, (cudaStream_t)stream, logits, (long long)ld,
+                       (int)vocab, (int)pad_idx, (int)eos_idx, (int)unk_idx, unk_penalty, (int)K, cand_val, (int*)cand_idx,
+                       eos_lprob, (const int*)ban_ids, (const int*)ban_n, (int)ban_ld));
   count_launch();
   return SB_OK;
 }
@@ -978,9 +1072,40 @@ extern "C" int sb_logits_topk_tiles(const float* logits, int64_t ld, const float
   const int n_tiles = (vocab + TKT_TILE - 1) / TKT_TILE;
   const size_t smem = (size_t)2 * n_tiles * sizeof(float);
   SB_REQUIRE(smem <= 40 * 1024, SB_ENOSUP, "sb_logits_topk_tiles: vocabulary of %d too large", vocab);
-  SB_CUDA_OK(launch_k(logits_topk_tiles_kernel, dim3(rows), dim3(TKT_THREADS), smem, (cudaStream_t)stream, logits, (long long)ld,
+  SB_CUDA_OK(launch_k(logits_topk_tiles_kernel<false>, dim3(rows), dim3(TKT_THREADS), smem, (cudaStream_t)stream, logits, (long long)ld,
                        (const float2*)tile_stats, (int)rows, (int)vocab, (int)pad_idx, (int)eos_idx, (int)unk_idx, unk_penalty, (int)K,
-                       cand_val, (int*)cand_idx, eos_lprob));
+                       cand_val, (int*)cand_idx, eos_lprob, (const int*)nullptr, (const int*)nullptr, 0));
+  count_launch();
+  return SB_OK;
+}
+
+extern "C" int sb_logits_topk_tiles_ban(const float* logits, int64_t ld, const float* tile_stats, int32_t rows, int32_t vocab,
+                                        int32_t pad_idx, int32_t eos_idx, int32_t unk_idx, float unk_penalty, int32_t K, float* cand_val,
+                                        int32_t* cand_idx, float* eos_lprob, const int32_t* ban_ids, const int32_t* ban_n,
+                                        int32_t ban_ld, sb_stream_t stream) {
+  using namespace sb;
+  SB_REQUIRE(logits && tile_stats && cand_val && cand_idx && eos_lprob && ban_ids && ban_n && rows > 0 && vocab > 0 && ban_ld > 0,
+             SB_EINVAL, "sb_logits_topk_tiles_ban: bad args");
+  SB_REQUIRE(K > 0 && K <= TK_MAX, SB_ENOSUP, "sb_logits_topk_tiles_ban: K=%d unsupported (<= %d)", K, TK_MAX);
+  SB_REQUIRE(ld % 4 == 0 && ((uintptr_t)logits % 16) == 0, SB_EINVAL, "sb_logits_topk_tiles_ban: logits must be 16-byte aligned rows");
+  const int n_tiles = (vocab + TKT_TILE - 1) / TKT_TILE;
+  const size_t smem = (size_t)2 * n_tiles * sizeof(float) + (size_t)(vocab + 31) / 32 * sizeof(unsigned);
+  SB_REQUIRE((size_t)2 * n_tiles * sizeof(float) <= 40 * 1024, SB_ENOSUP, "sb_logits_topk_tiles_ban: vocabulary of %d too large", vocab);
+  SB_CUDA_OK(allow_dynamic_smem(logits_topk_tiles_kernel<true>, smem));
+  SB_CUDA_OK(launch_k(logits_topk_tiles_kernel<true>, dim3(rows), dim3(TKT_THREADS), smem, (cudaStream_t)stream, logits, (long long)ld,
+                       (const float2*)tile_stats, (int)rows, (int)vocab, (int)pad_idx, (int)eos_idx, (int)unk_idx, unk_penalty, (int)K,
+                       cand_val, (int*)cand_idx, eos_lprob, (const int*)ban_ids, (const int*)ban_n, (int)ban_ld));
+  count_launch();
+  return SB_OK;
+}
+
+extern "C" int sb_ban_step(const int32_t* seqs, int32_t seq_ld, const int32_t* step_ptr, int32_t rows, const int32_t* table,
+                           int32_t cap, int32_t width, int32_t* ban_ids, int32_t* ban_n, sb_stream_t stream) {
+  using namespace sb;
+  SB_REQUIRE(seqs && step_ptr && table && ban_ids && ban_n && rows > 0 && seq_ld > 0 && cap > 0 && width > 0, SB_EINVAL,
+             "sb_ban_step: bad args");
+  SB_CUDA_OK(launch_k(ban_step_kernel, dim3(rows), dim3(256), 0, (cudaStream_t)stream, (const int*)seqs, (int)seq_ld,
+                       (const int*)step_ptr, (const int*)table, (int)cap, (int)width, (int*)ban_ids, (int*)ban_n));
   count_launch();
   return SB_OK;
 }

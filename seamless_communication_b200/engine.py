@@ -404,9 +404,24 @@ class UnitYEngine:
         check(lib.sb_store_step(h.buf.data_ptr(), st["hist"].data_ptr(), st["step"].data_ptr(), R * M * 2, stream), "sb_store_step")
         ops.gemm(h, w["text_embed"], c.text_vocab, None, out=st["logits"], out_f32=True, tile_stats=st["tile_stats"])
 
-    def _topk(self, st, eos_idx, unk_penalty):
-        """log-softmax statistics + top-K candidates of every row (st["logits"] / st["tile_stats"] of the last projection)."""
+    def _topk(self, st, eos_idx, unk_penalty, ban=False):
+        """log-softmax statistics + top-K candidates of every row (st["logits"] / st["tile_stats"] of the last projection).
+        `ban`: the ids sb_ban_step wrote to st["ban_ids"] are not candidates."""
         lib, c = _lib.load(), self.cfg
+        if ban:
+            b = st["ban"]
+            if st["tile_stats"] is not None:
+                check(lib.sb_logits_topk_tiles_ban(st["logits"].buf.data_ptr(), st["logits"].buf.stride(0), st["tile_stats"].data_ptr(),
+                                                   st["R"], c.text_vocab, c.text_pad, eos_idx, c.text_unk, unk_penalty, st["K"],
+                                                   st["cand_val"].data_ptr(), st["cand_idx"].data_ptr(), st["eos_lprob"].data_ptr(),
+                                                   b["ids"].data_ptr(), b["n"].data_ptr(), b["cap"], ops._stream()),
+                      "sb_logits_topk_tiles_ban")
+            else:
+                check(lib.sb_logits_topk_ban(st["logits"].buf.data_ptr(), st["logits"].buf.stride(0), st["R"], c.text_vocab, c.text_pad,
+                                             eos_idx, c.text_unk, unk_penalty, st["K"], st["cand_val"].data_ptr(),
+                                             st["cand_idx"].data_ptr(), st["eos_lprob"].data_ptr(), b["ids"].data_ptr(),
+                                             b["n"].data_ptr(), b["cap"], ops._stream()), "sb_logits_topk_ban")
+            return
         if st["tile_stats"] is not None:
             check(lib.sb_logits_topk_tiles(st["logits"].buf.data_ptr(), st["logits"].buf.stride(0), st["tile_stats"].data_ptr(), st["R"],
                                            c.text_vocab, c.text_pad, eos_idx, c.text_unk, unk_penalty, st["K"], st["cand_val"].data_ptr(),
@@ -416,10 +431,14 @@ class UnitYEngine:
                                      eos_idx, c.text_unk, unk_penalty, st["K"], st["cand_val"].data_ptr(),
                                      st["cand_idx"].data_ptr(), st["eos_lprob"].data_ptr(), ops._stream()), "sb_logits_topk")
 
-    def _decoder_step_select(self, st):
+    def _decoder_step_select(self, st, ban=False):
         lib = _lib.load()
         stream = ops._stream()
-        self._topk(st, self.cfg.text_eos, st["unk_penalty"])
+        if ban:
+            b = st["ban"]
+            check(lib.sb_ban_step(st["seqs"].data_ptr(), st["ML"], st["step"].data_ptr(), st["R"], b["table"].data_ptr(), b["cap"],
+                                  b["width"], b["ids"].data_ptr(), b["n"].data_ptr(), stream), "sb_ban_step")
+        self._topk(st, self.cfg.text_eos, st["unk_penalty"], ban=ban)
         check(lib.sb_beam_step(C.byref(st["beam_desc"]), stream), "sb_beam_step")
         check(lib.sb_step_advance(st["step"].data_ptr(), stream), "sb_step_advance")
 
@@ -503,8 +522,9 @@ class UnitYEngine:
         d.fin_anc, d.len_budget = fin["anc"].data_ptr(), st["budget"].data_ptr()
         st["beam_desc"] = d
         st["ds_launch"] = self._decoder_plan(st) if self.decode_fused else None
-        st["g_fwd"] = st["g_sel"] = None
-        st["n_fwd"] = st["n_sel"] = 0
+        st["g_fwd"] = st["g_sel"] = st["g_sel_ban"] = None
+        st["n_fwd"] = st["n_sel"] = st["n_sel_ban"] = 0
+        st["ban"], st["ban_on"] = None, False
         self._graphs[key] = st
         self._evict_search_states(keep=key)
         return st
@@ -620,6 +640,45 @@ class UnitYEngine:
             self._decoder_step_select(st)
         st["n_fwd"], st["n_sel"] = n1 - n0, ops.launch_count() - n1
 
+    def _capture_ban(self, st):
+        """Capture the select half with banned sequences (sb_ban_step, ban-aware top-K, sb_beam_step, sb_step_advance) on the
+        state's ban table; searches without bans keep replaying g_sel."""
+        with _CAPTURE_LOCK:
+            s = torch.cuda.Stream()
+            s.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(s):
+                self._decoder_step_select(st, ban=True)
+            torch.cuda.current_stream().wait_stream(s)
+            n0 = ops.launch_count()
+            st["g_sel_ban"] = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(st["g_sel_ban"], capture_error_mode="thread_local"):
+                self._decoder_step_select(st, ban=True)
+            st["n_sel_ban"] = ops.launch_count() - n0
+
+    def _set_bans(self, st, banned):
+        """Pack the banned sequences into the state's device table ([count][lengths x cap][cap rows of `width` tokens,
+        right-aligned]) with one asynchronous host-to-device copy.  The buffers, and the graph captured on them, are
+        replaced only when the table outgrows their capacity (both rounded up to a power of two)."""
+        n, width = len(banned), max(len(x) for x in banned)
+        b = st["ban"]
+        if b is None or n > b["cap"] or width > b["width"]:
+            cap = max(16, 1 << (max(n, b["cap"] if b else 0) - 1).bit_length())
+            w = max(8, 1 << (max(width, b["width"] if b else 0) - 1).bit_length())
+            dev = self.device
+            b = st["ban"] = dict(cap=cap, width=w, table=torch.zeros(1 + cap + cap * w, dtype=I32, device=dev),
+                                 ids=torch.zeros((st["R"], cap), dtype=I32, device=dev), n=torch.zeros(st["R"], dtype=I32, device=dev))
+            st["g_sel_ban"] = None
+        cap, w = b["cap"], b["width"]
+        host = torch.zeros(1 + cap + cap * w, dtype=I32, pin_memory=True)
+        host[0] = n
+        lens = host[1:1 + cap]
+        toks = host[1 + cap:].view(cap, w)
+        for j, seq in enumerate(banned):
+            lens[j] = len(seq)
+            toks[j, w - len(seq):] = torch.as_tensor(seq, dtype=I32)
+        b["table"].copy_(host, non_blocking=True)
+        b["host"] = host  # the pinned source stays alive until the copy has run
+
     def _search_reset(self, st, prefix):
         fin, P = st["fin"], st["P"]
         st["seqs"].zero_()
@@ -630,7 +689,8 @@ class UnitYEngine:
         fin["n_active"].fill_(st["B"])
         st["step"].zero_()
 
-    def _search_prepare(self, st, enc: Seq, enc_lens, prefix, len_penalty, unk_penalty, min_seq_len, use_graph, max_len):
+    def _search_prepare(self, st, enc: Seq, enc_lens, prefix, len_penalty, unk_penalty, min_seq_len, use_graph, max_len,
+                        banned=None):
         """(Re)initialise one cached search state in place for the sentences of `enc` and a length budget `max_len`
         (<= the state's allocated length); capture its graphs if needed."""
         c, M = self.cfg, self.M
@@ -640,8 +700,11 @@ class UnitYEngine:
         if st.get("opts_cap") != (min_seq_len, float(len_penalty)) or st.get("unk_cap") != float(unk_penalty):
             d.min_len, d.len_penalty = min_seq_len, len_penalty
             st["opts_cap"] = (min_seq_len, float(len_penalty))  # compared as Python values: c_float rounds 0.9 and would recapture every call
-            st["g_fwd"] = st["g_sel"] = None  # scalar options are baked into the captured select graph
+            st["g_fwd"] = st["g_sel"] = st["g_sel_ban"] = None  # scalar options are baked into the captured select graphs
             st["unk_cap"] = float(unk_penalty)
+        st["ban_on"] = bool(banned)
+        if banned:
+            self._set_bans(st, banned)
         if enc_lens is not None:
             st["enc_lens"].copy_(enc_lens)
         for i in range(c.dec_layers):
@@ -655,18 +718,22 @@ class UnitYEngine:
         if use_graph and st["g_fwd"] is None:
             self._capture(st)
             self._search_reset(st, prefix)  # the warm-up touched position-0 cache rows and the search state
+        if use_graph and banned and st["g_sel_ban"] is None:
+            self._capture_ban(st)
+            self._search_reset(st, prefix)
 
     def _search_step(self, st, use_graph, select=True):
+        ban = st["ban_on"]
         if use_graph:
             st["g_fwd"].replay()
             if select:
-                st["g_sel"].replay()
+                st["g_sel_ban" if ban else "g_sel"].replay()
             with self._count_lock:
-                self.graph_kernels += st["n_fwd"] + (st["n_sel"] if select else 0)
+                self.graph_kernels += st["n_fwd"] + ((st["n_sel_ban"] if ban else st["n_sel"]) if select else 0)
         else:
             self._decoder_step_forward(st)
             if select:
-                self._decoder_step_select(st)
+                self._decoder_step_select(st, ban=ban)
 
     def _search_bootstrap_step(self, st, prefix, i, use_graph):
         """fairseq2.cpp:1162-1247: feed prefix[i], score prefix[i+1] (the top-K kernel reports the lprob of its
@@ -714,12 +781,21 @@ class UnitYEngine:
 
     @torch.inference_mode()
     def beam_search(self, enc: Seq, enc_lens, prefix: List[int], beam=5, soft_max=(1, 200), hard_max=1024,
-                    len_penalty=1.0, unk_penalty=0.0, min_seq_len=1, use_graph=True, cross_kv=None, state_len=None):
+                    len_penalty=1.0, unk_penalty=0.0, min_seq_len=1, use_graph=True, cross_kv=None, state_len=None,
+                    banned=None):
         """Device-resident beam search (see _beam_search); runs on the thread's high-priority stream, ordered after the
         caller's stream on entry and before it on exit."""
         hp = self._priority_stream()
+        if banned is not None:
+            banned = [[int(t) for t in (x.tolist() if isinstance(x, torch.Tensor) else x)] for x in banned]
+            V = self.cfg.text_vocab
+            for x in banned:
+                if not x:
+                    raise ValueError("a banned sequence must not be empty")
+                if not all(0 <= t < V for t in x):
+                    raise ValueError(f"banned token ids must lie in [0, {V})")
         args = (enc, enc_lens, prefix, beam, soft_max, hard_max, len_penalty, unk_penalty, min_seq_len, use_graph, cross_kv,
-                state_len)
+                state_len, banned)
         if hp is None:
             return self._beam_search(*args)
         cur = torch.cuda.current_stream()
@@ -730,13 +806,16 @@ class UnitYEngine:
         return out
 
     def _beam_search(self, enc: Seq, enc_lens, prefix: List[int], beam=5, soft_max=(1, 200), hard_max=1024,
-                     len_penalty=1.0, unk_penalty=0.0, min_seq_len=1, use_graph=True, cross_kv=None, state_len=None):
+                     len_penalty=1.0, unk_penalty=0.0, min_seq_len=1, use_graph=True, cross_kv=None, state_len=None,
+                     banned=None):
         """Device-resident beam search.  Returns per sentence the finished hypotheses [(score, ids)], best first
         (semantics: fairseq2.cpp:1371-1608; see decode.cu).  `cross_kv` is ignored (kept for API stability): the
         static cross-attention K/V of the cached search state are recomputed from `enc`.
         `state_len`: allocate (and cache) the search state for this many positions instead of the length budget
         min(hard_max, a*S_enc + b); the budget is then a device scalar of the state, so searches whose budgets differ
-        share one state and its captured graphs.  None: the state is sized by the budget."""
+        share one state and its captured graphs.  None: the state is sized by the budget.
+        `banned`: token-id sequences of fairseq2's BannedSequenceProcessor, applied at every selecting step (not in the
+        prefix bootstrap): a row whose last n-1 tokens equal a sequence's first n-1 cannot take its last token."""
         M = self.M
         B, S_enc = enc.B, enc.T
         a, b = soft_max
@@ -759,7 +838,7 @@ class UnitYEngine:
             st = self._search_state(b1 - b0, S_enc, ML_state, beam, P, enc_lens is not None, use_graph, slot=g)
             e = enc if G == 1 else Seq(b1 - b0, S_enc, M, buf=enc.buf[b0 * S_enc:b1 * S_enc])
             self._search_prepare(st, e, None if enc_lens is None else enc_lens[b0:b1], prefix, len_penalty, unk_penalty,
-                                 min_seq_len, use_graph, ML)
+                                 min_seq_len, use_graph, ML, banned)
             st["b0"] = b0
             groups.append(st)
         n_steps = ML - 1 - (P - 1)

@@ -1,2 +1,2 @@
-from .generator import SequenceGeneratorOptions, UnitYGenerator
+from .generator import BannedSequenceProcessor, SequenceGeneratorOptions, UnitYGenerator
 from .translator import BatchedSpeechOutput, Modality, Task, Translator

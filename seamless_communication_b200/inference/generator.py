@@ -5,7 +5,7 @@ work behind them is the device-resident beam search and the NAR T2U of `engine.p
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Any, List, Optional, Tuple
+from typing import Any, List, Optional, Sequence, Tuple
 
 import torch
 from torch import Tensor
@@ -40,6 +40,24 @@ def filter_unit_ngrams(units: Tensor) -> Tensor:
     return torch.tensor(arr).to(units).unsqueeze(0)
 
 
+class BannedSequenceProcessor:
+    """fairseq2's `BannedSequenceProcessor`, the text step processor of the MinTox re-decode (toxicity/mintox.py): at
+    every selecting step of the search, a hypothesis whose last n-1 tokens equal the first n-1 tokens of a banned
+    sequence cannot take its last token (n = 1: never).  The search applies it on the device (engine.beam_search
+    `banned`, decode.cu sb_ban_step); this object only holds and checks the sequences."""
+
+    def __init__(self, banned_seqs: Sequence[Any]) -> None:
+        if not banned_seqs:
+            raise ValueError("`banned_seqs` must contain at least one element.")
+        seqs = []
+        for s in banned_seqs:
+            ids = [int(t) for t in (s.tolist() if isinstance(s, Tensor) else s)]
+            if not ids:
+                raise ValueError("a banned sequence must contain at least one token.")
+            seqs.append(ids)
+        self.banned_seqs: List[List[int]] = seqs
+
+
 @dataclass
 class SequenceGeneratorOptions:
     """generator.py:59-84 (same fields and defaults)."""
@@ -71,8 +89,9 @@ class UnitYGenerator:
         self.unit_opts = unit_opts or SequenceGeneratorOptions(soft_max_seq_len=(25, 50), hard_max_seq_len=5000)
         if model.text_decoder is None:
             raise ValueError("`UnitYGenerator` requires a text decoder, but the current UnitY model does not have one.")
-        if self.text_opts.step_processor is not None:
-            raise NotImplementedError("step processors (MinTox banned sequences) are outside the S2ST hot path")
+        p = self.text_opts.step_processor
+        if p is not None and not isinstance(p, BannedSequenceProcessor):
+            raise NotImplementedError("the text search supports BannedSequenceProcessor as its only step processor")
         self.text_tokenizer = text_tokenizer
         enc = text_tokenizer.create_encoder(task="translation", lang=target_lang, mode="target")
         self.prefix = enc.prefix_indices.tolist()  # [</s>, __lang__]
@@ -86,7 +105,7 @@ class UnitYGenerator:
             self.unit_decoder = unit_tokenizer.create_decoder()
             self.unit_prefix_indices = unit_tokenizer.create_encoder(lang=target_lang).prefix_indices
             if isinstance(model.t2u_model, UnitYT2UModel) and self.unit_opts.step_processor is not None:
-                raise NotImplementedError("step processors (MinTox banned sequences) are outside the S2ST hot path")
+                raise NotImplementedError("step processors are not supported on the unit search")
 
     @torch.inference_mode()
     def __call__(self, source_seqs: Tensor, source_padding_mask: Optional[PaddingMask], input_modality: str = "speech",
@@ -105,8 +124,10 @@ class UnitYGenerator:
         enc = Seq(B, S, M, buf=enc_out.view(B * S, M))
         enc_lens = None if enc_mask is None else enc_mask.seq_lens.to(device=enc_out.device, dtype=I32)
         o = self.text_opts
+        banned = o.step_processor.banned_seqs if o.step_processor is not None else None
         hyps = eng.beam_search(enc, enc_lens, self.prefix, beam=o.beam_size, soft_max=o.soft_max_seq_len,
-                               hard_max=o.hard_max_seq_len, len_penalty=o.len_penalty, unk_penalty=o.unk_penalty)
+                               hard_max=o.hard_max_seq_len, len_penalty=o.len_penalty, unk_penalty=o.unk_penalty,
+                               banned=banned)
         for h in hyps:
             if not h:
                 raise RuntimeError("The sequence generator returned no hypothesis at index 0. Please file a bug report.")

@@ -44,13 +44,19 @@ class Translator:
 
     def __init__(self, model_name_or_card: Union[str, UnitYModel], vocoder_name_or_card: Union[str, Vocoder, None], device,
                  text_tokenizer=None, apply_mintox: bool = False, dtype=torch.float16,
-                 input_modality: Optional[Modality] = None, output_modality: Optional[Modality] = None, **model_kw):
+                 input_modality: Optional[Modality] = None, output_modality: Optional[Modality] = None,
+                 bad_word_checker=None, **model_kw):
+        """`apply_mintox`: re-decode the rows whose translation adds toxicity with the added words banned (MinTox,
+        toxicity/mintox.py).  It needs `bad_word_checker`, the checker of `toxicity.load_etox_bad_word_checker`: the
+        reference downloads the word lists from the card, this implementation reads a local copy."""
         self.device = torch.device(device)
         if self.device.type != "cuda":
             # the reference silently switches to fp32 on CPU (translator.py:110-111); this implementation has no CPU path
             raise RuntimeError("seamless_communication_b200.Translator needs a CUDA device (sm_90a); no CPU fallback exists.")
-        if apply_mintox:
-            raise NotImplementedError("MinTox re-decoding is outside the S2ST hot path (SURVEY.md 2.1 P14)")
+        if apply_mintox and bad_word_checker is None:
+            raise ValueError("apply_mintox=True needs bad_word_checker=load_etox_bad_word_checker('mintox', dataset_dir=...) "
+                             "(seamless_communication_b200.toxicity): the ETOX word lists are not downloaded")
+        self.bad_word_checker = bad_word_checker if apply_mintox else None
         with_t2u = output_modality != Modality.TEXT  # translator.py:105-107
         if isinstance(model_name_or_card, UnitYModel):
             self.model = model_name_or_card
@@ -151,6 +157,7 @@ class Translator:
                                           "encoder), which is not implemented; S2ST, S2TT and ASR are")
         if self.apply_mintox and not (src_lang is not None or src_text is not None):
             raise ValueError("`src_lang` must be specified when `apply_mintox` is `True` or you need to specify src_text.")
+        mintox = self.apply_mintox and task_str.upper() != Task.ASR.name
         if isinstance(input, dict):
             src = cast(SequenceData, input)
         elif input_modality == Modality.SPEECH:
@@ -177,13 +184,17 @@ class Translator:
                                            input_modality, output_modality, tgt_lang, text_generation_opts,
                                            unit_generation_opts, unit_generation_ngram_filtering=unit_generation_ngram_filtering,
                                            duration_factor=duration_factor, prosody_encoder_input=prosody_encoder_input)
+        unit_lens = self._tls.generator.last_unit_output["unit_lens"] if output_modality == Modality.SPEECH else None
+        if mintox:
+            texts, units, unit_lens = self._mintox(src, input_modality, output_modality, src_lang, tgt_lang, src_text, texts,
+                                                   units, unit_lens, text_generation_opts, unit_generation_opts,
+                                                   unit_generation_ngram_filtering, duration_factor, prosody_encoder_input)
         if output_modality == Modality.TEXT:
             return texts, None
         assert units is not None and self.model.t2u_model is not None
         pad_idx = self.model.t2u_model.target_vocab_info.pad_idx
         if isinstance(self.model.t2u_model, UnitYT2UModel):
-            return texts, self._speech_output_ar(units, self._tls.generator.last_unit_output["unit_lens"], tgt_lang, spkr,
-                                                 sample_rate)
+            return texts, self._speech_output_ar(units, unit_lens, tgt_lang, spkr, sample_rate)
         # translator.py:396-404 incl. the quirk that a genuine unit 1 is dropped like a pad (SURVEY a16)
         units_host = units.cpu()
         speech_units = [u[u != pad_idx].tolist() for u in units_host]
@@ -194,6 +205,28 @@ class Translator:
                 n = int(wav.size(-1) * len(speech_units[i]) / len(units[i]))
                 audio_wavs.append(wav[i, :, :n].unsqueeze(0))
         return texts, BatchedSpeechOutput(units=speech_units, audio_wavs=audio_wavs, sample_rate=sample_rate)
+
+    def _mintox(self, src, input_modality, output_modality, src_lang, tgt_lang, src_text, texts, units, unit_lens, text_opts,
+                unit_opts, ngram_filtering, duration_factor, prosody_encoder_input):
+        """translator.py:335-380.  Without `src_text` the reference transcribes the input with
+        predict(input, "ASR", tgt_lang=tgt_lang) and the same options: the same search over the same input from the same
+        prefix as the pass just run, so its texts are reused instead of searched again."""
+        from ..toxicity.mintox import mintox_pipeline
+        if src_text is not None:
+            if len(texts) != 1:
+                raise ValueError(f"src_text is one source text, but the batch has {len(texts)} rows")
+            src_texts = [src_text]
+        else:
+            src_texts = list(texts)
+        texts, units, rows = mintox_pipeline(self.model, self.text_tokenizer, self.unit_tokenizer, self.device, src_lang, tgt_lang,
+                                             src, input_modality, output_modality, src_texts, texts, units, ngram_filtering,
+                                             text_opts, unit_opts, self.bad_word_checker, duration_factor, prosody_encoder_input)
+        if rows and isinstance(unit_lens, list):  # AR T2U: _speech_output_ar reads each row's own unit count
+            new_lens = self._tls.generator.last_unit_output["unit_lens"]
+            unit_lens = list(unit_lens)
+            for j, i in enumerate(rows):
+                unit_lens[i] = new_lens[j]
+        return texts, units, unit_lens
 
     def _speech_output_ar(self, units: Tensor, unit_lens: List[int], tgt_lang: str, spkr: Optional[int],
                           sample_rate: int) -> BatchedSpeechOutput:

@@ -382,6 +382,27 @@ class SyntheticNllbTokenizer:
     def create_decoder(self):
         return _TextDecoder(self)
 
+    def create_raw_encoder(self, *, device=None):
+        """Encoder without prefix or suffix tokens (fairseq2 `create_raw_encoder`, used by MinTox to encode banned words).
+        A word encodes to its "▁"-piece, or to UNK when the inventory lacks it.  A leading "★" becomes a token of its own
+        (UNK: the inventory has no such piece) followed by the rest of the word, so that encode("★" + w)[1:] is w's
+        encoding, as MinTox expects of a SentencePiece model."""
+        return _RawTextEncoder(self, device)
+
+
+class _RawTextEncoder(_TextEncoder):
+    def __init__(self, tok: "SyntheticNllbTokenizer", device):
+        super().__init__(tok, [], [], device)
+
+    def __call__(self, text: str) -> torch.Tensor:
+        ids = []
+        for w in text.strip().split():
+            if w.startswith("\u2605") and len(w) > 1:
+                ids.append(self.tok.vocab_info.unk_idx)
+                w = w[1:]
+            ids.append(self.tok.model.token_to_index(SPACE + w))
+        return torch.tensor(ids, dtype=torch.int64, device=self.device)
+
 
 class SyntheticCharTokenizer:
     """Char-level piece model (reference: models/unity/char_tokenizer.py:30; vocab 10943 for v2)."""
