@@ -254,72 +254,6 @@ typedef struct {
 int sb_beam_step(const sb_beam_t* p, sb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
- * sb_decoder_step - module-level entry: ONE persistent kernel for a whole incremental decoder step over `rows`
- * hypotheses (embedding frontend -> every pre-LN decoder layer with KV cache -> final LayerNorm).
- * Replaces: TransformerEmbeddingFrontend + StandardTransformerDecoder.forward with an IncrementalStateBag as driven by
- * UnitYX2TModel.decode (models/unity/model.py:233-252); C++ mirror StandardTransformerDecoderLayer_forward
- * (ggml/examples/unity/fairseq2.cpp:979-1094), TransformerEmbeddingFrontend_forward (:917-953).
- * Workspace convention of SURVEY 8(b): sb_decoder_plan_query() reports every size, the caller allocates, then
- * sb_decoder_plan_init() fills the POD launch descriptor (shapes, pointers and TMA descriptors travel as kernel
- * parameters; no device allocation, no copy) that sb_decoder_step() replays (graph-capturable: a memset node + one
- * kernel).  At most 32 layers.
- * Weights keep the reference layouts (Linear (out,in) fp16) but are STACKED into two tensors so that one TMA descriptor
- * serves all layers: w_dim_stack [layers][3*dim (q|k|v) + dim (self out) + dim (cross q) + dim (cross out) + ffn_dim
- * (FFN inner)][dim] and w_ffn_stack [layers][dim][ffn_dim] (FFN out); biases / LayerNorm fp32 per layer.
- * State per call: x (residual stream), h (= LN of x, at the end: the decoder output of this step), both [rows][dim].
- * ---------------------------------------------------------------------------------------------------------------- */
-typedef struct {
-  /* biases of: self qkv, self out, cross q, cross out, FFN inner, FFN out */
-  const float *qkv_b, *out_b, *cq_b, *co_b, *ffn1_b, *ffn2_b;
-  const float *ca_ln_w, *ca_ln_b;     /* encoder_decoder_attn_layer_norm */
-  const float *ffn_ln_w, *ffn_ln_b;   /* ffn_layer_norm */
-  const float *next_ln_w, *next_ln_b; /* next layer's self_attn_layer_norm, or the decoder's final layer_norm */
-  void *k_cache, *v_cache;            /* fp16 [rows (slots)][heads][max_len][64]: position `step` is written at slot = row */
-  const void *cross_k, *cross_v;      /* fp16 [batch][heads][s_enc][64] static encoder K / V of this layer (sb_kv_heads_major) */
-} sb_decoder_layer_t;
-
-typedef struct {
-  int32_t layers, dim, ffn_dim, heads, rows, beam, groups /* 0 = auto */, max_len, s_enc;
-  const sb_decoder_layer_t* layer;    /* [layers] (host array) */
-  const void *w_dim_stack, *w_ffn_stack; /* stacked fp16 weights, see above */
-  const float *ln0_w, *ln0_b;         /* layer 0 self_attn_layer_norm */
-  const void* embed;                  /* fp16 [vocab][dim] */
-  const float* pos;                   /* fp32 [>= max_len][dim] sinusoid table (position index = step) */
-  float embed_scale;
-  const int32_t* seqs; int32_t seqs_ld;   /* token of row r at position *step_ptr: seqs[r*seqs_ld + step] */
-  const int32_t* anc; int32_t anc_ld;     /* cache slot of row r at position t < step: anc[r*anc_ld + t] */
-  const int32_t* step_ptr;
-  const int32_t* enc_lens;            /* [batch] or NULL */
-  void *x, *h, *att, *ffn_act;        /* fp16 [rows][dim] x3, [rows][ffn_dim] */
-  float* part_qkv; int64_t part_qkv_floats;
-  float* part; int64_t part_floats;
-  void* hist;                         /* fp16 [max_len][rows][dim] or NULL: h of every step */
-  uint32_t* counters; int64_t counters_len;
-  uint64_t* timeline;                 /* NULL, or [groups][n_phases][8] ns stamps of CTA 0 (profiling) */
-} sb_decoder_plan_desc_t;
-
-typedef struct {
-  int64_t part_qkv_floats, part_floats, counters_len;
-  int32_t groups, rows_per_group, npad, ctas_per_group, stages, smem_bytes, n_phases;
-  int32_t splits[6];                  /* split-K of qkv, out, cq, co, ffn1 (always 1), ffn2 */
-} sb_decoder_plan_info_t;
-
-typedef struct {
-  uint32_t* counters; int64_t counters_len;
-  int32_t grid, block, smem_bytes, cooperative, npad, reserved;
-  uint64_t params[768];               /* opaque: the kernel's parameter block (shapes, pointers, 5 TMA descriptors) */
-} sb_decoder_launch_t;
-
-/* kv [batch*s_enc][ld] with K | V concatenated along the features (the output of the cross-attention k/v projection)
- * -> head-major k_out, v_out [batch][heads][s_enc][64]: the keys of one (utterance, head) become consecutive rows */
-int sb_kv_heads_major(const void* kv, int64_t ld, int32_t batch, int32_t s_enc, int32_t heads, void* k_out, void* v_out,
-                      sb_stream_t stream);
-int sb_decoder_plan_query(int32_t layers, int32_t dim, int32_t ffn_dim, int32_t rows, int32_t beam, int32_t groups,
-                          sb_decoder_plan_info_t* info);
-int sb_decoder_plan_init(const sb_decoder_plan_desc_t* desc, sb_decoder_launch_t* launch);
-int sb_decoder_step(const sb_decoder_launch_t* launch, sb_stream_t stream);
-
-/* ------------------------------------------------------------------------------------------------------------------
  * NAR T2U frontend (models/unity/nar_decoder_frontend.py:130-334, length_regulator.py:24-39,275-321) on device.
  * ---------------------------------------------------------------------------------------------------------------- */
 /* text ids -> per-subword char lengths + char id sequence, using per-token tables built once from the vocab:

@@ -48,38 +48,6 @@ class BeamDesc(C.Structure):
     ]
 
 
-class DecoderLayerDesc(C.Structure):
-    _fields_ = [(n, c_p) for n in (
-        "qkv_b", "out_b", "cq_b", "co_b", "ffn1_b", "ffn2_b",
-        "ca_ln_w", "ca_ln_b", "ffn_ln_w", "ffn_ln_b", "next_ln_w", "next_ln_b", "k_cache", "v_cache", "cross_k", "cross_v")
-    ]
-
-
-class DecoderPlanDesc(C.Structure):
-    _fields_ = [
-        ("layers", i32), ("dim", i32), ("ffn_dim", i32), ("heads", i32), ("rows", i32), ("beam", i32), ("groups", i32),
-        ("max_len", i32), ("s_enc", i32),
-        ("layer", C.POINTER(DecoderLayerDesc)), ("w_dim_stack", c_p), ("w_ffn_stack", c_p), ("ln0_w", c_p), ("ln0_b", c_p), ("embed", c_p), ("pos", c_p),
-        ("embed_scale", f32), ("seqs", c_p), ("seqs_ld", i32), ("anc", c_p), ("anc_ld", i32), ("step_ptr", c_p),
-        ("enc_lens", c_p), ("x", c_p), ("h", c_p), ("att", c_p), ("ffn_act", c_p),
-        ("part_qkv", c_p), ("part_qkv_floats", i64), ("part", c_p), ("part_floats", i64), ("hist", c_p),
-        ("counters", c_p), ("counters_len", i64), ("timeline", c_p),
-    ]
-
-
-class DecoderPlanInfo(C.Structure):
-    _fields_ = [
-        ("part_qkv_floats", i64), ("part_floats", i64), ("counters_len", i64),
-        ("groups", i32), ("rows_per_group", i32), ("npad", i32), ("ctas_per_group", i32), ("stages", i32),
-        ("smem_bytes", i32), ("n_phases", i32), ("splits", i32 * 6),
-    ]
-
-
-class DecoderLaunch(C.Structure):
-    _fields_ = [("counters", c_p), ("counters_len", i64), ("grid", i32), ("block", i32),
-                ("smem_bytes", i32), ("cooperative", i32), ("npad", i32), ("reserved", i32), ("params", C.c_uint64 * 768)]
-
-
 # name -> argtypes (restype is int unless listed in _RESTYPES); must list every symbol include/seamless_b200.h declares
 PROTOTYPES = {
     "sb_last_error": [],
@@ -111,10 +79,6 @@ PROTOTYPES = {
     "sb_ban_step": [c_p, i32, c_p, i32, c_p, i32, i32, c_p, c_p, c_p],
     "sb_logits_topk_ban": [c_p, i64, i32, i32, i32, i32, i32, f32, i32, c_p, c_p, c_p, c_p, c_p, i32, c_p],
     "sb_logits_topk_tiles_ban": [c_p, i64, c_p, i32, i32, i32, i32, i32, f32, i32, c_p, c_p, c_p, c_p, c_p, i32, c_p],
-    "sb_kv_heads_major": [c_p, i64, i32, i32, i32, c_p, c_p, c_p],
-    "sb_decoder_plan_query": [i32, i32, i32, i32, i32, i32, C.POINTER(DecoderPlanInfo)],
-    "sb_decoder_plan_init": [C.POINTER(DecoderPlanDesc), C.POINTER(DecoderLaunch)],
-    "sb_decoder_step": [C.POINTER(DecoderLaunch), c_p],
     "sb_text_to_chars": [c_p, i32, i32, c_p, c_p, c_p, i32, i32, i32, i32, c_p, c_p, i32, c_p, c_p],
     "sb_upsample_add": [c_p, i32, i32, i32, c_p, c_p, i32, i32, i32, i32, i32, c_p, c_p, c_p, c_p, i32, f32, c_p, c_p],
     "sb_durations": [c_p, i32, i32, c_p, f32, i32, c_p, i32, i32, f32, c_p, c_p],

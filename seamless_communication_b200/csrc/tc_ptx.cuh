@@ -1,5 +1,4 @@
-// wgmma / TMA / mbarrier PTX wrappers shared by the sm_90a tensor-core kernels (gemm_tcgen05.cu, decode_gemm.cu,
-// decoder_step.cu).
+// wgmma / TMA / mbarrier PTX wrappers shared by the sm_90a tensor-core kernels (gemm_tcgen05.cu, decode_gemm.cu).
 #pragma once
 #include "common.cuh"
 
@@ -278,11 +277,6 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, const void* 
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ unsigned long long gtime_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
 }
 
 }  // namespace sb

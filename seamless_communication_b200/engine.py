@@ -61,6 +61,8 @@ def _interleave_glu(w: torch.Tensor) -> torch.Tensor:
 
 
 class UnitYEngine:
+    decode_fused = False  # bench.py reads it for its decoder-step label: every step is the per-op launch chain
+
     def __init__(self, cfg: UnitYConfig, state_dict: Dict[str, torch.Tensor], tokenizers, device="cuda"):
         _lib.require_cuda()
         self.cfg = cfg
@@ -78,21 +80,13 @@ class UnitYEngine:
         if self.has_t2u:
             self._build_char_tables()
         self._graphs = collections.OrderedDict()
-        self._search_streams = []
         # lanes (parallel.LanePool): several host threads drive independent batches on their own streams; each thread
         # sees its own search states / graphs (the lane is part of the cache key) and its own "last search" record
         self._tls = threading.local()
         self._count_lock = threading.Lock()
-        self.search_priority = os.environ.get("SB_SEARCH_PRIORITY", "0") != "0"
         self._state_lock = threading.RLock()
-        self.search_groups = 1  # concurrent sentence groups in beam_search (see _search_group_count)
         self.decode_prefetch = os.environ.get("SB_DECODE_PREFETCH", "1") != "0"
         self.graph_kernels = 0  # kernels executed through CUDA-graph replays (bench.py: gpu_launches)
-        # SB_DECODER_FUSED=1: one persistent kernel per decoder step (sb_decoder_step, csrc/decoder_step.cu) instead of the
-        # per-op launch chain.  Opt-in (correct and deterministic, not timed on H100): a grid-wide phase barrier through L2
-        # costs about as much as a kernel boundary inside a CUDA graph, so the fusion saves launches but not waiting.
-        self.decode_fused = os.environ.get("SB_DECODER_FUSED", "0") != "0"
-        self.decode_timeline = os.environ.get("SB_DS_TIMELINE", "0") != "0"
         # all six weight products of a decoder step on the transposed wgmma kernel (decode_gemm.cu) at <= 256 rows;
         # SB_DECODE_GEMM_T=0 selects the row-major wgmma chain instead
         self.decode_gemm_t = os.environ.get("SB_DECODE_GEMM_T", "1") != "0"
@@ -189,23 +183,6 @@ class UnitYEngine:
             ln(f"{p}.encoder_decoder_attn_layer_norm"); mha(f"{p}.encoder_decoder_attn", fuse_qkv=False)
             ln(f"{p}.ffn_layer_norm"); lin(f"{p}.ffn.inner_proj"); lin(f"{p}.ffn.output_proj")
         ln("text_decoder.layer_norm")
-        # The persistent decoder-step kernel (csrc/decoder_step.cu) reads all layers through two TMA descriptors: stack the
-        # decoder matrices with K = model_dim ([layer][q|k|v, self out, cross q, cross out, FFN inner]) and the FFN output
-        # matrices (K = ffn_dim); the per-layer entries of `w` become views of the stacks (no second copy).
-        M_, F_ = c.model_dim, c.dec_ffn_dim
-        names = (".self_attn.qkv", ".self_attn.output_proj", ".encoder_decoder_attn.q_proj", ".encoder_decoder_attn.output_proj",
-                 ".ffn.inner_proj")
-        self.dec_w_dim = torch.empty((c.dec_layers * (6 * M_ + F_), M_), dtype=F16, device=dev)
-        self.dec_w_ffn = torch.empty((c.dec_layers * M_, F_), dtype=F16, device=dev)
-        for i in range(c.dec_layers):
-            p, r = f"text_decoder.layers.{i}", i * (6 * M_ + F_)
-            for n in names:
-                t = w[p + n + ".w"]
-                self.dec_w_dim[r:r + t.shape[0]].copy_(t)
-                w[p + n + ".w"] = self.dec_w_dim[r:r + t.shape[0]]
-                r += t.shape[0]
-            self.dec_w_ffn[i * M_:(i + 1) * M_].copy_(w[p + ".ffn.output_proj.w"])
-            w[p + ".ffn.output_proj.w"] = self.dec_w_ffn[i * M_:(i + 1) * M_]
         if self.has_t2u_encoder:
             for i in range(c.t2u_enc_layers):
                 p = f"t2u_model.encoder.layers.{i}"
@@ -356,11 +333,6 @@ class UnitYEngine:
         R, stream = st["R"], ops._stream()
         x, h, part = st["x"], st["h"], st["partials"]
         w = self.w
-        if st.get("ds_launch") is not None:
-            # embedding frontend + all decoder layers + final LayerNorm (+ hist[step] = h) in one persistent kernel
-            check(lib.sb_decoder_step(C.byref(st["ds_launch"]), stream), "sb_decoder_step")
-            ops.gemm(h, w["text_embed"], c.text_vocab, None, out=st["logits"], out_f32=True, tile_stats=st["tile_stats"])
-            return
         check(lib.sb_embed_step(st["seqs"].data_ptr(), st["ML"], st["step"].data_ptr(), w["text_embed"].data_ptr(),
                                 self.pos.data_ptr(), math.sqrt(M), x.buf.data_ptr(), R, M, stream), "sb_embed_step")
         self._ln(x, "text_decoder.layers.0.self_attn_layer_norm", out=h)
@@ -451,22 +423,22 @@ class UnitYEngine:
         self._tls.lane = int(lane)
 
     @property
-    def _last_search_states(self):
-        return getattr(self._tls, "last_states", [])
+    def _last_search_state(self):
+        return getattr(self._tls, "last_state", None)
 
-    @_last_search_states.setter
-    def _last_search_states(self, groups):
-        self._tls.last_states = groups
+    @_last_search_state.setter
+    def _last_search_state(self, st):
+        self._tls.last_state = st
 
-    def _search_state(self, B, S_enc, ML, beam, P, has_lens, use_graph, slot=0):
+    def _search_state(self, B, S_enc, ML, beam, P, has_lens, use_graph):
         with self._state_lock:  # the cache is shared by the lanes' host threads
-            return self._search_state_locked(B, S_enc, ML, beam, P, has_lens, use_graph, slot)
+            return self._search_state_locked(B, S_enc, ML, beam, P, has_lens, use_graph)
 
-    def _search_state_locked(self, B, S_enc, ML, beam, P, has_lens, use_graph, slot):
+    def _search_state_locked(self, B, S_enc, ML, beam, P, has_lens, use_graph):
         """Static buffers + captured CUDA graphs of one decoder step, cached per problem shape so that repeated
         predict() calls replay the same graphs (the reference rebuilds its generator per call, translator.py:179-186;
         construction here stays cheap after the first call)."""
-        key = (B, S_enc, ML, beam, P, has_lens, use_graph, slot, self.decode_fused, self.decode_gemm_t, self.lane)
+        key = (B, S_enc, ML, beam, P, has_lens, use_graph, self.decode_gemm_t, self.lane)
         st = self._graphs.get(key)
         if st is not None:
             self._graphs.move_to_end(key)
@@ -521,7 +493,6 @@ class UnitYEngine:
         d.fin_seqs, d.active, d.n_active = fin["seqs"].data_ptr(), fin["active"].data_ptr(), fin["n_active"].data_ptr()
         d.fin_anc, d.len_budget = fin["anc"].data_ptr(), st["budget"].data_ptr()
         st["beam_desc"] = d
-        st["ds_launch"] = self._decoder_plan(st) if self.decode_fused else None
         st["g_fwd"] = st["g_sel"] = st["g_sel_ban"] = None
         st["n_fwd"] = st["n_sel"] = st["n_sel_ban"] = 0
         st["ban"], st["ban_on"] = None, False
@@ -562,61 +533,10 @@ class UnitYEngine:
         for k in list(self._graphs.keys()):
             if total <= budget or len(self._graphs) <= 1:
                 break
-            if k == keep or any(k is not keep and st is self._graphs[k] for st in (getattr(self, "_last_search_states", None) or [])):
+            if k == keep or self._graphs[k] is self._last_search_state:
                 continue
             total -= sizes[k]
             del self._graphs[k]
-
-    def _decoder_plan(self, st):
-        """Device-side plan of the persistent decoder-step kernel for one search state (workspace sizes come from
-        sb_decoder_plan_query; every pointer in the plan is a static buffer of `st`)."""
-        lib = _lib.load()
-        c, M, dev, w = self.cfg, self.M, self.device, self.w
-        info = _lib.DecoderPlanInfo()
-        check(lib.sb_decoder_plan_query(c.dec_layers, M, c.dec_ffn_dim, st["R"], st["beam"], 0, C.byref(info)), "sb_decoder_plan_query")
-        st["ds_info"] = info
-        st["ds_part_qkv"] = torch.empty(int(info.part_qkv_floats), dtype=torch.float32, device=dev)
-        st["ds_part"] = torch.empty(int(info.part_floats), dtype=torch.float32, device=dev)
-        st["ds_counters"] = torch.zeros(int(info.counters_len), dtype=I32, device=dev)
-        # head-major copies of the static encoder K / V ([B][H][S_enc][64]); the self-attention cache is head-major as well
-        # ([slot][H][max_len][64], same bytes as st["kc"] / st["vc"]): one hypothesis reads a few contiguous runs
-        B = st["B"]
-        st["cross_k_hm"] = [torch.empty((B, self.H, st["S_enc"], 64), dtype=F16, device=dev) for _ in range(c.dec_layers)]
-        st["cross_v_hm"] = [torch.empty((B, self.H, st["S_enc"], 64), dtype=F16, device=dev) for _ in range(c.dec_layers)]
-        st["ds_timeline"] = (torch.zeros((int(info.groups), int(info.n_phases), 8), dtype=torch.int64, device=dev)
-                             if self.decode_timeline else None)
-        layers = (_lib.DecoderLayerDesc * c.dec_layers)()
-        for i in range(c.dec_layers):
-            p, L = f"text_decoder.layers.{i}", layers[i]
-            last = i + 1 == c.dec_layers
-            nxt = "text_decoder.layer_norm" if last else f"text_decoder.layers.{i + 1}.self_attn_layer_norm"
-            for field, name in (("qkv", ".self_attn.qkv"), ("out", ".self_attn.output_proj"),
-                                ("cq", ".encoder_decoder_attn.q_proj"), ("co", ".encoder_decoder_attn.output_proj"),
-                                ("ffn1", ".ffn.inner_proj"), ("ffn2", ".ffn.output_proj")):
-                setattr(L, field + "_b", w[p + name + ".b"].data_ptr())
-            L.ca_ln_w, L.ca_ln_b = (w[p + ".encoder_decoder_attn_layer_norm" + s].data_ptr() for s in (".w", ".b"))
-            L.ffn_ln_w, L.ffn_ln_b = (w[p + ".ffn_layer_norm" + s].data_ptr() for s in (".w", ".b"))
-            L.next_ln_w, L.next_ln_b = w[nxt + ".w"].data_ptr(), w[nxt + ".b"].data_ptr()
-            L.k_cache, L.v_cache = st["kc"][i].data_ptr(), st["vc"][i].data_ptr()
-            L.cross_k, L.cross_v = st["cross_k_hm"][i].data_ptr(), st["cross_v_hm"][i].data_ptr()
-        d = _lib.DecoderPlanDesc()
-        d.layers, d.dim, d.ffn_dim, d.heads, d.rows, d.beam, d.groups = c.dec_layers, M, c.dec_ffn_dim, self.H, st["R"], st["beam"], int(info.groups)
-        d.max_len, d.s_enc = st["ML"], st["S_enc"]
-        d.layer = layers
-        d.w_dim_stack, d.w_ffn_stack = self.dec_w_dim.data_ptr(), self.dec_w_ffn.data_ptr()
-        d.ln0_w, d.ln0_b = (w["text_decoder.layers.0.self_attn_layer_norm" + s].data_ptr() for s in (".w", ".b"))
-        d.embed, d.pos, d.embed_scale = w["text_embed"].data_ptr(), self.pos.data_ptr(), math.sqrt(M)
-        d.seqs, d.seqs_ld, d.anc, d.anc_ld = st["seqs"].data_ptr(), st["ML"], st["anc"].data_ptr(), st["ML"]
-        d.step_ptr, d.enc_lens = st["step"].data_ptr(), ops._p(st["enc_lens"])
-        d.x, d.h, d.att, d.ffn_act = (st[k].buf.data_ptr() for k in ("x", "h", "att", "ffn"))
-        d.part_qkv, d.part_qkv_floats = st["ds_part_qkv"].data_ptr(), int(info.part_qkv_floats)
-        d.part, d.part_floats = st["ds_part"].data_ptr(), int(info.part_floats)
-        d.hist = st["hist"].data_ptr()
-        d.counters, d.counters_len = st["ds_counters"].data_ptr(), int(info.counters_len)
-        d.timeline = ops._p(st["ds_timeline"])
-        launch = _lib.DecoderLaunch()
-        check(lib.sb_decoder_plan_init(C.byref(d), C.byref(launch)), "sb_decoder_plan_init")
-        return launch
 
     def _capture(self, st):
         """Capture the forward and the select halves of a decoder step (all pointers/shapes static)."""
@@ -709,11 +629,6 @@ class UnitYEngine:
             st["enc_lens"].copy_(enc_lens)
         for i in range(c.dec_layers):
             self._lin(enc, f"text_decoder.layers.{i}.encoder_decoder_attn.kv", 2 * M, out=st["cross_kv"][i])
-            if st.get("ds_launch") is not None:
-                kv = st["cross_kv"][i].buf
-                check(_lib.load().sb_kv_heads_major(kv.data_ptr(), kv.stride(0), st["B"], st["S_enc"], self.H,
-                                                    st["cross_k_hm"][i].data_ptr(), st["cross_v_hm"][i].data_ptr(), ops._stream()),
-                      "sb_kv_heads_major")
         self._search_reset(st, prefix)
         if use_graph and st["g_fwd"] is None:
             self._capture(st)
@@ -759,55 +674,10 @@ class UnitYEngine:
         st["best_fin"] = best
         return results
 
-    def _search_group_count(self, B: int) -> int:
-        """Sentences are searched independently (no cross-sentence op, SURVEY 8e), so the batch can be cut into groups
-        whose step chains run concurrently on separate streams.  Every group re-reads the decoder weights and the chains
-        contend for the same SMs, so the default is one group (more groups are not timed on H100); SB_SEARCH_GROUPS
-        overrides."""
-        g = int(os.environ.get("SB_SEARCH_GROUPS", "0")) or self.search_groups
-        return max(1, min(g, B // 4)) if B >= 8 else 1
-
-    def _priority_stream(self):
-        """The calling thread's high-priority stream for the search (SB_SEARCH_PRIORITY=1; default off).  The idea: a
-        decoder step is a chain of ~260 dependent kernels of a few microseconds, and when other lanes (parallel.LanePool)
-        have long GEMM grids of the encoder / T2U / vocoder queued, a high-priority step kernel could take the next free
-        SM slots instead of waiting behind them.  Not timed on H100, so the search stays on the caller's stream."""
-        if not self.search_priority:
-            return None
-        s = getattr(self._tls, "hp_stream", None)
-        if s is None:
-            s = self._tls.hp_stream = torch.cuda.Stream(device=self.device, priority=-1)
-        return s
-
     @torch.inference_mode()
     def beam_search(self, enc: Seq, enc_lens, prefix: List[int], beam=5, soft_max=(1, 200), hard_max=1024,
                     len_penalty=1.0, unk_penalty=0.0, min_seq_len=1, use_graph=True, cross_kv=None, state_len=None,
                     banned=None):
-        """Device-resident beam search (see _beam_search); runs on the thread's high-priority stream, ordered after the
-        caller's stream on entry and before it on exit."""
-        hp = self._priority_stream()
-        if banned is not None:
-            banned = [[int(t) for t in (x.tolist() if isinstance(x, torch.Tensor) else x)] for x in banned]
-            V = self.cfg.text_vocab
-            for x in banned:
-                if not x:
-                    raise ValueError("a banned sequence must not be empty")
-                if not all(0 <= t < V for t in x):
-                    raise ValueError(f"banned token ids must lie in [0, {V})")
-        args = (enc, enc_lens, prefix, beam, soft_max, hard_max, len_penalty, unk_penalty, min_seq_len, use_graph, cross_kv,
-                state_len, banned)
-        if hp is None:
-            return self._beam_search(*args)
-        cur = torch.cuda.current_stream()
-        hp.wait_stream(cur)
-        with torch.cuda.stream(hp):
-            out = self._beam_search(*args)
-        cur.wait_stream(hp)
-        return out
-
-    def _beam_search(self, enc: Seq, enc_lens, prefix: List[int], beam=5, soft_max=(1, 200), hard_max=1024,
-                     len_penalty=1.0, unk_penalty=0.0, min_seq_len=1, use_graph=True, cross_kv=None, state_len=None,
-                     banned=None):
         """Device-resident beam search.  Returns per sentence the finished hypotheses [(score, ids)], best first
         (semantics: fairseq2.cpp:1371-1608; see decode.cu).  `cross_kv` is ignored (kept for API stability): the
         static cross-attention K/V of the cached search state are recomputed from `enc`.
@@ -816,7 +686,14 @@ class UnitYEngine:
         share one state and its captured graphs.  None: the state is sized by the budget.
         `banned`: token-id sequences of fairseq2's BannedSequenceProcessor, applied at every selecting step (not in the
         prefix bootstrap): a row whose last n-1 tokens equal a sequence's first n-1 cannot take its last token."""
-        M = self.M
+        if banned is not None:
+            banned = [[int(t) for t in (x.tolist() if isinstance(x, torch.Tensor) else x)] for x in banned]
+            V = self.cfg.text_vocab
+            for x in banned:
+                if not x:
+                    raise ValueError("a banned sequence must not be empty")
+                if not all(0 <= t < V for t in x):
+                    raise ValueError(f"banned token ids must lie in [0, {V})")
         B, S_enc = enc.B, enc.T
         a, b = soft_max
         ML = hard_max if a <= 0 else min(hard_max, int(a * S_enc) + b)  # fairseq2.cpp:1097-1105
@@ -827,63 +704,22 @@ class UnitYEngine:
                              f"({self.cfg.max_seq_len}), but is {ML} instead.")
         assert enc.PH == 0 and enc.Tp == enc.T, "encoder output must be a halo-free Seq"
         ML_state = ML if state_len is None else max(ML, int(state_len))
-        G = self._search_group_count(B)
-        bounds = [(B * g) // G for g in range(G + 1)]
-        main = torch.cuda.current_stream()
-        while len(self._search_streams) < G:
-            self._search_streams.append(torch.cuda.Stream())
-        groups = []
-        for g in range(G):
-            b0, b1 = bounds[g], bounds[g + 1]
-            st = self._search_state(b1 - b0, S_enc, ML_state, beam, P, enc_lens is not None, use_graph, slot=g)
-            e = enc if G == 1 else Seq(b1 - b0, S_enc, M, buf=enc.buf[b0 * S_enc:b1 * S_enc])
-            self._search_prepare(st, e, None if enc_lens is None else enc_lens[b0:b1], prefix, len_penalty, unk_penalty,
-                                 min_seq_len, use_graph, ML, banned)
-            st["b0"] = b0
-            groups.append(st)
+        st = self._search_state(B, S_enc, ML_state, beam, P, enc_lens is not None, use_graph)
+        self._search_prepare(st, enc, enc_lens, prefix, len_penalty, unk_penalty, min_seq_len, use_graph, ML, banned)
         n_steps = ML - 1 - (P - 1)
-        if G == 1:
-            st = groups[0]
-            for i in range(P - 1):
-                self._search_bootstrap_step(st, prefix, i, use_graph)
-            done = 0
-            while done < n_steps:
-                chunk = min(32, n_steps - done)
-                for _ in range(chunk):
-                    self._search_step(st, use_graph)
-                done += chunk
-                if done < n_steps and int(st["fin"]["n_active"].item()) == 0:
-                    break
-        else:
-            streams = self._search_streams[:G]
-            for s in streams:
-                s.wait_stream(main)
-            for i in range(P - 1):
-                for st, s in zip(groups, streams):
-                    with torch.cuda.stream(s):
-                        self._search_bootstrap_step(st, prefix, i, use_graph)
-            live, done = list(range(G)), 0
-            while done < n_steps and live:
-                chunk = min(32, n_steps - done)
-                for _ in range(chunk):
-                    for g in live:  # interleaved so that the groups' step chains overlap on the device
-                        with torch.cuda.stream(streams[g]):
-                            self._search_step(groups[g], use_graph)
-                done += chunk
-                if done < n_steps:
-                    still = []
-                    for g in live:
-                        with torch.cuda.stream(streams[g]):
-                            if int(groups[g]["fin"]["n_active"].item()) != 0:
-                                still.append(g)
-                    live = still
-            for s in streams:
-                main.wait_stream(s)
-        results = []
-        for st in groups:
-            results.extend(self._search_collect(st))
-        groups[0]["enc_ptr"] = enc.buf.data_ptr() if G == 1 else None
-        self._last_search_states = groups
+        for i in range(P - 1):
+            self._search_bootstrap_step(st, prefix, i, use_graph)
+        done = 0
+        while done < n_steps:
+            chunk = min(32, n_steps - done)
+            for _ in range(chunk):
+                self._search_step(st, use_graph)
+            done += chunk
+            if done < n_steps and int(st["fin"]["n_active"].item()) == 0:
+                break
+        results = self._search_collect(st)
+        st["enc_ptr"] = enc.buf.data_ptr()
+        self._last_search_state = st
         return results
 
     @torch.inference_mode()
@@ -892,19 +728,16 @@ class UnitYEngine:
         beam search (position t of a hypothesis lives in hist[t][slot_t]).  Same function of the same tokens as the
         reference's teacher-forced re-run of the decoder over the winning sequence minus its final EOS
         (inference/generator.py:281-299), without the second pass.  `lengths[b]` = len(hypothesis) - 1."""
-        groups = getattr(self, "_last_search_states", None)
-        if not groups or any(j < 0 for st in groups for j in st["best_fin"]):
+        st = self._last_search_state
+        if st is None or any(j < 0 for j in st["best_fin"]):
             return None
         M, dev = self.M, self.device
         B, L = len(lengths), max(lengths)
         t_idx = torch.arange(L, device=dev)[None, :]
-        parts = []
-        for st in groups:
-            Bg = st["B"]
-            sel = torch.tensor(st["best_fin"], dtype=torch.int64, device=dev)
-            slots = st["fin"]["anc"][torch.arange(Bg, device=dev), sel][:, :L].to(torch.int64)  # (Bg, L)
-            parts.append(st["hist"][t_idx.expand(Bg, L), slots])                                 # (Bg, L, M) row gather
-        out = parts[0] if len(parts) == 1 else torch.cat(parts)
+        Bs = st["B"]
+        sel = torch.tensor(st["best_fin"], dtype=torch.int64, device=dev)
+        slots = st["fin"]["anc"][torch.arange(Bs, device=dev), sel][:, :L].to(torch.int64)  # (Bs, L)
+        out = st["hist"][t_idx.expand(Bs, L), slots]                                         # (Bs, L, M) row gather
         lens = torch.tensor(lengths, dtype=I32, device=dev)
         out = out * (t_idx < lens[:, None].to(torch.int64))[:, :, None].to(out.dtype)             # zero the padding rows
         return Seq(B, L, M, lens=lens, buf=out.reshape(B * L, M).contiguous())
@@ -916,8 +749,7 @@ class UnitYEngine:
         c, M, H = self.cfg, self.M, self.H
         B, L = text_seqs.shape
         if cross_kv is None:
-            sts = getattr(self, "_last_search_states", None)
-            st = sts[0] if sts and len(sts) == 1 else None
+            st = self._last_search_state
             cross_kv = st["cross_kv"] if (st is not None and st.get("enc_ptr") == enc.buf.data_ptr()) else self._cross_kv(enc)
         xb = ops.embed_seq(text_seqs.to(I32).contiguous(), self.w["text_embed"], self.pos, math.sqrt(M), M)
         x = Seq(B, L, M, lens=text_lens, buf=xb)

@@ -109,7 +109,7 @@ def test_bit_identical_to_row_major_kernels_at_step_slices(ops, rows):
     assert torch.equal(got.buf, want.buf)
 
 
-def test_search_step_transposed_equals_launch_chain():
+def test_search_step_transposed_equals_row_major_chain():
     """A beam search of 32 sentences x beam 5 (160 rows, the bench's step) on `small`: the default path (all six products
     on sb_gemm_decode) against decode_gemm_t = False (the row-major chain), at the same K slices: the hypotheses,
     their scores and the final-LayerNorm state of every step are identical; and a second default search is too."""
@@ -123,13 +123,13 @@ def test_search_step_transposed_equals_launch_chain():
     lens = torch.randint(3, S_enc + 1, (B,), dtype=torch.int32, device=dev)
     lens[0] = S_enc
     prefix = [cfg.text_eos, eng.text_tokenizer.lang_index("spa")]
-    assert eng.decode_gemm_t and not eng.decode_fused
+    assert eng.decode_gemm_t
     runs = {}
     try:
         for gemm_t in (True, False, True):
             eng.decode_gemm_t = gemm_t
             hyps = eng.beam_search(e, lens, prefix, beam=beam, soft_max=(1, 9), hard_max=40)
-            st = eng._last_search_states[0]
+            st = eng._last_search_state
             assert st["gemm_t"] == gemm_t and st["R"] == 160
             n = min(len(h[0][1]) for h in hyps) - 1
             run = (hyps, st["hist"][:n].clone())

@@ -424,78 +424,6 @@ def test_harvested_decoder_states_equal_teacher_forced_pass(tiny):
         assert got.buf.view(3, -1, M)[i, n:].abs().sum() == 0
 
 
-def test_beam_search_sentence_groups_on_streams_equal_single_group(tiny, monkeypatch):
-    """beam_search cuts the batch into sentence groups stepped concurrently on separate streams; hypotheses, scores and
-    harvested decoder states must not depend on the grouping."""
-    from seamless_communication_b200.ops import Seq
-    cfg, eng = tiny["cfg"], tiny["model"].engine
-    torch.manual_seed(11)
-    M, S_enc, B = cfg.model_dim, 10, 9
-    e = Seq(B, S_enc, M, buf=torch.randn(B * S_enc, M, device=dev).half())
-    lens = torch.tensor([10, 4, 10, 7, 10, 10, 2, 9, 10], dtype=torch.int32, device=dev)
-    prefix = [cfg.text_eos, tiny["toks"][0].lang_index("spa")]
-    out = {}
-    for g in (1, 2, 3):
-        monkeypatch.setenv("SB_SEARCH_GROUPS", str(g))
-        hyps = eng.beam_search(e, lens, prefix, beam=4, soft_max=(1, 6))
-        states = eng.harvest_decoder_states([len(h[0][1]) - 1 for h in hyps])
-        out[g] = (hyps, states.buf.clone())
-    assert len(eng._last_search_states) == 2  # 9 sentences: at most B // 4 groups
-    for g in (2, 3):
-        for h1, hg in zip(out[1][0], out[g][0]):
-            assert [x[1] for x in h1] == [x[1] for x in hg]
-            assert np.allclose([x[0] for x in h1], [x[0] for x in hg], rtol=0, atol=1e-6)
-        assert torch.equal(out[1][1], out[g][1])
-
-
-@pytest.mark.parametrize("which", ["tiny", "small"])
-def test_persistent_decoder_step_equals_launch_chain(tiny, small, which):
-    """sb_decoder_step (one persistent kernel per step: csrc/decoder_step.cu) against the per-op launch chain it
-    replaces, on the same search: the final-LayerNorm state of every step within fp16 accumulation-order noise, the
-    same hypotheses (or a margin-audited near tie), and the K/V cache written identically up to rounding."""
-    from seamless_communication_b200.ops import Seq
-    eng = (tiny["model"] if which == "tiny" else small).engine
-    cfg = eng.cfg
-    torch.manual_seed(21)
-    M, S_enc, B, beam = cfg.model_dim, 13, (7 if which == "tiny" else 32), 5
-    e = Seq(B, S_enc, M, buf=torch.randn(B * S_enc, M, device=dev).half())
-    lens = torch.randint(3, S_enc + 1, (B,), dtype=torch.int32, device=dev)
-    lens[0] = S_enc
-    prefix = [cfg.text_eos, eng.text_tokenizer.lang_index("spa")]
-    out = {}
-    old = eng.decode_fused
-    try:
-        for fused in (False, True):
-            eng.decode_fused = fused
-            hyps = eng.beam_search(e, lens, prefix, beam=beam, soft_max=(1, 9), hard_max=40)
-            st = eng._last_search_states[0]
-            assert (st["ds_launch"] is not None) == fused
-            n = min(len(h[0][1]) for h in hyps) - 1
-            kc = st["kc"][cfg.dec_layers - 1]
-            R = st["R"]
-            # the launch chain keeps K time-major [t][slot][M], the persistent kernel head-major [slot][head][t][64]
-            kc = (kc.view(R, eng.H, st["ML"], 64).permute(2, 0, 1, 3).reshape(st["ML"], R, M) if fused else kc)[:n]
-            out[fused] = (hyps, st["hist"][:n].clone(), kc.clone())
-    finally:
-        eng.decode_fused = old
-    (h0, hist0, kc0), (h1, hist1, kc1) = out[False], out[True]
-    # step 0..1 see identical inputs on both paths (same prefix): states agree to accumulation-order noise
-    assert rel(hist1[:2], hist0[:2]) < 4e-3 and rel(kc1[:2], kc0[:2]) < 4e-3
-    same = sum(a[0][1] == b[0][1] for a, b in zip(h0, h1))
-    assert same >= B - max(1, B // 8), f"only {same}/{B} best hypotheses agree"
-    for a, b in zip(h0, h1):
-        assert abs(a[0][0] - b[0][0]) < 2e-2
-    # determinism of the persistent kernel: a second search is bit-identical
-    eng.decode_fused = True
-    try:
-        hyps2 = eng.beam_search(e, lens, prefix, beam=beam, soft_max=(1, 9), hard_max=40)
-        st = eng._last_search_states[0]
-        assert [h[0][1] for h in hyps2] == [h[0][1] for h in h1]
-        assert torch.equal(st["hist"][:hist1.shape[0]], hist1)
-    finally:
-        eng.decode_fused = old
-
-
 def _teacher_forced_score(eng, e, lens, i, ids):
     """_oracle_score computed by the device: mean log-probability of ids[1:] under decode_full over sentence i."""
     from seamless_communication_b200 import ops
@@ -516,14 +444,14 @@ def _split_rel(got, want, n):
 
 
 @pytest.mark.parametrize("which", ["tiny", "small"])
-def test_long_search_states_equal_teacher_forced_pass(tiny, small, which, monkeypatch):
+def test_long_search_row_major_and_transposed_states_equal_teacher_forced_pass(tiny, small, which):
     """Searches at Translator.predict's default lengths (soft_max (1, 200), hard_max 1024) over 190 encoder frames:
     max_len 390, and min_seq_len 300 keeps every hypothesis alive past position 300.  This runs the step's attention
     past 128 positions and 128 frames - the ancestry slots past 128, the cross kernel's staging tail and > 48 KB shared
-    memory, the persistent kernel's attention in several passes (and, with SB_DS_STAGES=2, in passes of 24 keys) - on
-    all three step variants: the launch chain, the transposed decode GEMM and the persistent kernel.
+    memory - on both step variants: the row-major launch chain and the transposed decode GEMM.
     (a) The harvested states of every winner equal decode_full over the same ids, (b) on tiny also the oracle's fp32
-    teacher-forced decoder, (c) the variants pick the same winners up to near ties, (d) each variant is deterministic."""
+    teacher-forced decoder, (c) the transposed GEMM picks the same winners as the row-major chain up to near ties,
+    (d) each variant is deterministic."""
     from seamless_communication_b200.ops import Seq
     model = tiny["model"] if which == "tiny" else small
     eng = model.engine
@@ -535,23 +463,18 @@ def test_long_search_states_equal_teacher_forced_pass(tiny, small, which, monkey
     prefix = [cfg.text_eos, eng.text_tokenizer.lang_index("spa")]
     kw = dict(beam=beam, soft_max=(1, 200), hard_max=1024, min_seq_len=300)
     e_cpu = e.buf.view(B, S_enc, M).float().cpu()
-    variants = {"chain": (False, False), "gemm_t": (False, True), "fused": (True, False), "fused_stages2": (True, False)}
-    old = (eng.decode_fused, eng.decode_gemm_t)
+    variants = {"chain": False, "gemm_t": True}
+    old = eng.decode_gemm_t
     runs = {}
     try:
-        for name, (fused, gemm_t) in variants.items():
-            eng.decode_fused, eng.decode_gemm_t = fused, gemm_t
-            if name == "fused_stages2":  # a persistent-kernel plan with a 2-stage ring: self-attention passes of 24 keys
-                monkeypatch.setenv("SB_DS_STAGES", "2")
-                eng._graphs.clear()
+        for name, gemm_t in variants.items():
+            eng.decode_gemm_t = gemm_t
             reps = []
             for _ in range(2):
                 hyps = eng.beam_search(e, lens, prefix, **kw)
-                st = eng._last_search_states[0]
+                st = eng._last_search_state
                 assert st["ML"] == 390
-                assert st["gemm_t"] == gemm_t and (st["ds_launch"] is not None) == fused
-                if name == "fused_stages2":
-                    assert st["ds_info"].stages == 2
+                assert st["gemm_t"] == gemm_t
                 seqs = [h[0][1] for h in hyps]
                 assert all(len(s) >= 302 for s in seqs)
                 states = eng.harvest_decoder_states([len(s) - 1 for s in seqs]).buf.view(B, -1, M).clone()
@@ -581,34 +504,31 @@ def test_long_search_states_equal_teacher_forced_pass(tiny, small, which, monkey
                     lo, hi = _split_rel(s0[i], o, n)
                     print(f"{which} {name} sentence {i}: vs fp32 oracle rel {lo:.2e} (< 128) {hi:.2e} (>= 128)")
                     assert lo < 5e-3 and hi < 5e-3, (name, i, lo, hi)
-            if name == "fused_stages2":
-                monkeypatch.delenv("SB_DS_STAGES")
-                eng._graphs.clear()
     finally:
-        eng.decode_fused, eng.decode_gemm_t = old
-    # (c) the variants agree with the launch chain: same winners up to near ties
+        eng.decode_gemm_t = old
+    # (c) the transposed GEMM agrees with the row-major chain: same winners up to near ties
     h_ref, s_ref, _ = runs["chain"]
-    for name in ("gemm_t", "fused", "fused_stages2"):
-        h_v, s_v, _ = runs[name]
-        differ = 0
-        for i in range(B):
-            a, b = h_ref[i][0], h_v[i][0]
-            assert abs(a[0] - b[0]) < 2e-2, (name, i, a[0], b[0])
-            if a[1] != b[1]:
-                # margin audit: both winners score within a near tie under one teacher-forced scoring of the same
-                # sentence (the fp32 oracle on tiny; on small, which has no oracle fixture, the device's decode_full)
-                differ += 1
-                if uo is not None:
-                    e_i = e_cpu[i:i + 1, :int(lens[i])]
-                    sa, sb = _oracle_score(uo, e_i, a[1]), _oracle_score(uo, e_i, b[1])
-                else:
-                    sa, sb = (_teacher_forced_score(eng, e, lens, i, ids) for ids in (a[1], b[1]))
-                print(f"{which} {name} sentence {i}: winners differ, teacher-forced scores {sa:.5f} / {sb:.5f}")
-                assert abs(sa - sb) < 2e-2, (name, i, sa, sb)
+    name = "gemm_t"
+    h_v, s_v, _ = runs[name]
+    differ = 0
+    for i in range(B):
+        a, b = h_ref[i][0], h_v[i][0]
+        assert abs(a[0] - b[0]) < 2e-2, (name, i, a[0], b[0])
+        if a[1] != b[1]:
+            # margin audit: both winners score within a near tie under one teacher-forced scoring of the same
+            # sentence (the fp32 oracle on tiny; on small, which has no oracle fixture, the device's decode_full)
+            differ += 1
+            if uo is not None:
+                e_i = e_cpu[i:i + 1, :int(lens[i])]
+                sa, sb = _oracle_score(uo, e_i, a[1]), _oracle_score(uo, e_i, b[1])
             else:
-                lo, hi = _split_rel(s_v[i], s_ref[i], len(a[1]) - 1)
-                print(f"{which} {name} sentence {i}: states vs launch chain rel {lo:.2e} (< 128) {hi:.2e} (>= 128)")
-        print(f"{which} {name}: {differ}/{B} winners differ from the launch chain")
+                sa, sb = (_teacher_forced_score(eng, e, lens, i, ids) for ids in (a[1], b[1]))
+            print(f"{which} {name} sentence {i}: winners differ, teacher-forced scores {sa:.5f} / {sb:.5f}")
+            assert abs(sa - sb) < 2e-2, (name, i, sa, sb)
+        else:
+            lo, hi = _split_rel(s_v[i], s_ref[i], len(a[1]) - 1)
+            print(f"{which} {name} sentence {i}: states vs row-major chain rel {lo:.2e} (< 128) {hi:.2e} (>= 128)")
+    print(f"{which} {name}: {differ}/{B} winners differ from the row-major chain")
 
 
 def test_search_longer_than_position_table_is_refused(small):

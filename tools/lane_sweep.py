@@ -15,7 +15,6 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--lanes", default="1,2,3,4,6")
     ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--priority", default="1", help="comma list of SB_SEARCH_PRIORITY settings (engine.search_priority)")
     a = ap.parse_args()
     import bench
     from seamless_communication_b200 import synthetic as S
@@ -36,8 +35,7 @@ def main():
     torch.cuda.synchronize()
     enc, _ = eng.encode_speech(tr.fbank_batch(waves)["seqs"], None)
     main_stream = torch.cuda.current_stream()
-    for prio, L in [(int(p), int(v)) for p in a.priority.split(",") for v in a.lanes.split(",")]:
-        eng.search_priority = bool(prio)
+    for L in [int(v) for v in a.lanes.split(",")]:
         pool = LanePool(device, L, [eng])
         t0 = time.time()
         pool.warm(step)
@@ -60,7 +58,7 @@ def main():
         same = all(o[0] == texts0 for o in outs)
         ms = e0.elapsed_time(e1)
         ms_search = bench.lanes_search_ms(pool, eng, enc, L)
-        print(f"priority {prio} lanes {L}: {n} steps in {ms:.1f} ms (wall {wall * 1e3:.1f}) = {ms / n:.1f} ms/step, {32 * n / ms * 1e3:.1f} utt/s; "
+        print(f"lanes {L}: {n} steps in {ms:.1f} ms (wall {wall * 1e3:.1f}) = {ms / n:.1f} ms/step, {32 * n / ms * 1e3:.1f} utt/s; "
               f"texts identical to serial: {same}; {L} searches alone: {ms_search:.1f} ms; warm {t_warm:.1f}s; "
               f"mem {torch.cuda.max_memory_allocated() / 2**30:.1f} GiB", flush=True)
         pool.close()

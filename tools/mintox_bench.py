@@ -49,7 +49,7 @@ plain = Translator(model, voc, device="cuda")
 src = plain.fbank_batch(S.make_waveforms(args.batch, 160000, seed=1234).cuda())
 texts, _ = plain.predict(src, "s2st", "spa", text_generation_opts=opts)
 eng = model.engine
-st = eng._last_search_states[0]
+st = eng._last_search_state
 prefix = [cfg.text_eos, toks[0].lang_index("spa")]
 
 # ---- 1. select half per step

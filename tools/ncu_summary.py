@@ -73,7 +73,7 @@ def main():
                    f"{g['tensor'] / g['n']:9.1f}")
     # the beam search = launches from the first embedding-frontend kernel to the last step-advance kernel
     names = [x["name"] for x in seq]
-    first = next((i for i, n in enumerate(names) if n.startswith(("embed_kernel", "decoder_step_kernel"))), None)
+    first = next((i for i, n in enumerate(names) if n.startswith("embed_kernel")), None)
     last = max((i for i, n in enumerate(names) if n.startswith("step_advance_kernel")), default=None)
     dram = None
     if first is not None and last is not None and last > first:
