@@ -31,7 +31,8 @@ enum {
   SB_ENOSUP = -3   /* shape not supported by the kernels */
 };
 
-enum { SB_ACT_NONE = 0, SB_ACT_RELU = 1, SB_ACT_SILU = 2, SB_ACT_LRELU = 3, SB_ACT_TANH = 4 };
+/* SB_ACT_GELU: exact erf form, 0.5 x (1 + erf(x / sqrt 2)) (torch.nn.functional.gelu's default) */
+enum { SB_ACT_NONE = 0, SB_ACT_RELU = 1, SB_ACT_SILU = 2, SB_ACT_LRELU = 3, SB_ACT_TANH = 4, SB_ACT_GELU = 5 };
 
 const char* sb_last_error(void);
 int sb_version(void);
@@ -154,6 +155,45 @@ int sb_attention_relpos(const void* q, int64_t q_ld, const void* k, int64_t k_ld
                         int64_t out_ld, int32_t batch, int32_t heads, int32_t s, int32_t q_rows, int32_t q_halo,
                         int32_t kv_rows, int32_t kv_halo, const int32_t* kv_lens, const void* r, int64_t r_ld,
                         const float* u, const float* v_bias, sb_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * XLS-R unit extractor (wav2vec2 encoder + k-means, models/unit_extractor/unit_extractor.py:62-98).
+ * ---------------------------------------------------------------------------------------------------------------- */
+/* sb_w2v2_front - waveform statistics fused with feature-extractor layer 0.
+ *   Row b holds num_samples[b] = L samples of `wave` (row stride wave_ld); an odd L gets one appended sample of value
+ *   1.0 (Collater pad_to_multiple=2, pad_value=1), Lp = L + (L & 1).  The row is normalised over its Lp samples
+ *   (F.layer_norm over the whole sequence: biased variance, eps 1e-5, no affine; statistics in fp64), then
+ *   Conv1d(1 -> 512, k10, s5, bias) -> LayerNorm(512, eps 1e-5, affine) -> GELU (exact erf), fp32 throughout.
+ *   out: fp16 [batch][out_rows][512]; frame t < (Lp - 10) / 5 + 1 of row b at row b*out_rows + t, every other row of
+ *   the block written as 0.  No sample at index >= L of a row is read.  w0 fp32 [512][10], b0 / ln_w / ln_b fp32 [512];
+ *   stats: fp32 [batch][2] scratch (mean, 1/std).  Only frames t < out_rows are written (the caller sizes out_rows); a row
+ *   with fewer than 10 samples has no frame. */
+int sb_w2v2_front(const float* wave, int64_t wave_ld, const int32_t* num_samples, int32_t batch, const float* w0,
+                  const float* b0, const float* ln_w, const float* ln_b, void* out, int32_t out_rows, float* stats,
+                  sb_stream_t stream);
+/* sb_layernorm_gelu - sb_layernorm without residual, followed by GELU (exact erf) before the fp16 rounding: the
+ * LayerNorm -> GELU pair after every convolution of the wav2vec2 feature extractor.  Masked rows are written as 0. */
+int sb_layernorm_gelu(const void* x, void* y, const float* w, const float* b, int32_t dim, int32_t batch, int32_t T,
+                      int32_t in_rows, int32_t in_halo, int32_t out_rows, int32_t out_halo, const int32_t* lens,
+                      int32_t mask_out, sb_stream_t stream);
+/* sb_attention_hd80 - sb_attention's layouts and key-mask contract at head_dim 80 (16 heads x 80 = 1280 of XLS-R):
+ * scores = q.k^T * 80^-0.5, key mask j < kv_lens[b] (NULL: j < sk), no bias, no causal mode; a row with no admissible
+ * key is written as 0.  Columns [0, heads*80) of rows [q_halo, q_halo + sq) of each sequence of out are written.
+ * SB_ENOSUP unless q_ld, k_ld, v_ld are multiples of 8 elements and out_ld is even. */
+int sb_attention_hd80(const void* q, int64_t q_ld, const void* k, int64_t k_ld, const void* v, int64_t v_ld, void* out,
+                      int64_t out_ld, int32_t batch, int32_t heads, int32_t sq, int32_t sk, int32_t q_rows, int32_t q_halo,
+                      int32_t kv_rows, int32_t kv_halo, const int32_t* kv_lens, sb_stream_t stream);
+/* sb_nearest_centroid - KmeansModel.forward (kmeans.py:25-30) without the distance matrix:
+ *   units[r] = argmin_c (|c|^2 - 2 x_r . c), ties to the lowest c; |x_r|^2 is the same for every c of a row, so dropping
+ *   it does not change the argmin.  One sb_gemm of x (rows, dim) fp16 against the centroids (K, dim) fp16 whose
+ *   epilogue keeps the per-row, per-tile (min, argmin) and folds it into `best` with a 64-bit atomicMin on (orderable
+ *   float bits << 32 | index), so the result is the same in every launch order.  No output tile is written.
+ *   neg_half_norm fp32 [K] = -|c|^2 / 2 (the caller computes |c|^2 in fp64 from the fp16 centroids).
+ *   Row r is valid when seq_rows == 0 or r % seq_rows < seq_lens[r / seq_rows]; invalid rows get unit -1.
+ *   best: uint64 [rows] scratch; units: int32 [rows]. */
+int sb_nearest_centroid(const void* x, int64_t x_ld, int32_t rows, int32_t dim, const void* centroids, const float* neg_half_norm,
+                        int32_t K, int32_t seq_rows, const int32_t* seq_lens, uint64_t* best, int32_t* units,
+                        sb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * sb_dwconv_ln_silu - Conformer conv module middle: causal depthwise Conv1d(k) -> LayerNorm(C) -> SiLU.

@@ -156,6 +156,57 @@ class VocoderConfig:
         return asdict(self)
 
 
+@dataclass
+class Wav2Vec2EncoderConfig:
+    """The wav2vec2 encoder fields the unit extractor reads (reference models/unit_extractor/wav2vec2_layer_output.py:23-54
+    `_encoder_xlsr2_1b_v2`): a 7-layer conv feature extractor with LayerNorm after every conv, a grouped positional conv
+    and pre-LN Transformer encoder layers with GELU FFNs.  Head dim and channels per positional-conv group are 80 in every
+    named configuration (the attention kernel is specialised for head_dim 80)."""
+
+    name: str = "xlsr2_1b_v2"
+    model_dim: int = 1280
+    max_seq_len: int = 4096
+    feature_dim: int = 512
+    feature_extractor_layer_descs: Tuple[Tuple[int, int, int], ...] = ((512, 10, 5),) + ((512, 3, 2),) * 4 + ((512, 2, 2),) * 2
+    feature_extractor_bias: bool = True
+    feature_extractor_layer_norm_convs: bool = True
+    pos_encoder_type: str = "conv"
+    pos_encoder_depth: int = 1
+    pos_conv_kernel_size: int = 128
+    num_pos_conv_groups: int = 16
+    use_conformer: bool = False
+    num_encoder_layers: int = 48
+    num_encoder_attn_heads: int = 16
+    ffn_inner_dim: int = 5120
+    norm_order: str = "PRE"
+
+    @property
+    def head_dim(self) -> int:
+        return self.model_dim // self.num_encoder_attn_heads
+
+    def to_dict(self) -> Dict:
+        return asdict(self)
+
+
+def xlsr2_1b_v2() -> Wav2Vec2EncoderConfig:
+    return Wav2Vec2EncoderConfig()
+
+
+def tiny_xlsr() -> Wav2Vec2EncoderConfig:
+    """Test copy: 320 wide, 4 heads of 80, 4 positional-conv groups of 80 channels, 4 layers; full feature extractor."""
+    return Wav2Vec2EncoderConfig(name="tiny_xlsr", model_dim=320, num_pos_conv_groups=4, num_encoder_layers=4,
+                                 num_encoder_attn_heads=4, ffn_inner_dim=1280)
+
+
+def small_xlsr() -> Wav2Vec2EncoderConfig:
+    """Test copy: 640 wide, 8 heads of 80, 8 positional-conv groups, 6 layers."""
+    return Wav2Vec2EncoderConfig(name="small_xlsr", model_dim=640, num_pos_conv_groups=8, num_encoder_layers=6,
+                                 num_encoder_attn_heads=8, ffn_inner_dim=2560)
+
+
+WAV2VEC2_ARCHS = {"xlsr2_1b_v2": xlsr2_1b_v2, "tiny_xlsr": tiny_xlsr, "small_xlsr": small_xlsr}
+
+
 def base_v2() -> UnitYConfig:
     return UnitYConfig()
 

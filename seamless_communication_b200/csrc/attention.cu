@@ -583,6 +583,136 @@ __global__ void __launch_bounds__(128, 2) attention2_kernel(const AttnArgs p) {
     }
 }
 
+// ---- head_dim 80 (XLS-R, 16 x 80 = 1280): attention_kernel's plain path with five 16-wide k-steps for Q.K^T and ten 8-wide
+// output tiles for P.V; rows padded to 88 halves (176 B, an odd multiple of 16 B: conflict-free ldmatrix).
+constexpr int HD80 = 80;
+constexpr int LDS80 = HD80 + 8;
+
+__global__ void __launch_bounds__(128) attention_hd80_kernel(const AttnArgs p) {
+  extern __shared__ __align__(16) uint8_t smem_attn[];
+  elem_t* sQ = reinterpret_cast<elem_t*>(smem_attn);  // [AQ][LDS80]
+  elem_t* sK = sQ + AQ * LDS80;                       // [AK][LDS80]
+  elem_t* sV = sK + AK * LDS80;                       // [AK][LDS80]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = lane >> 2, tq = lane & 3;
+  const int q0 = blockIdx.x * AQ;
+  const int h = blockIdx.y, b = blockIdx.z;
+  const int kv_len = p.kv_lens ? min(p.kv_lens[b], p.sk) : p.sk;
+  const float scale = 0.11180339887498948f;  // 80^-0.5
+
+  for (int i = threadIdx.x; i < AQ * (HD80 / 8); i += blockDim.x) {
+    const int r = i / (HD80 / 8), c = (i % (HD80 / 8)) * 8;
+    uint4 u = make_uint4(0, 0, 0, 0);
+    if (q0 + r < p.sq) u = *reinterpret_cast<const uint4*>(p.q + ((long long)b * p.q_rows + p.q_halo + q0 + r) * p.q_ld + h * HD80 + c);
+    *reinterpret_cast<uint4*>(sQ + r * LDS80 + c) = u;
+  }
+  __syncthreads();
+  uint32_t qa[5][4];
+#pragma unroll
+  for (int ks = 0; ks < 5; ++ks) {
+    const elem_t* ptr = sQ + (warp * 16 + (lane & 7) + 8 * ((lane >> 3) & 1)) * LDS80 + ks * 16 + 8 * (lane >> 4);
+    ldsm_x4(qa[ks][0], qa[ks][1], qa[ks][2], qa[ks][3], ptr);
+  }
+  float o[10][4];
+#pragma unroll
+  for (int i = 0; i < 10; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+  float mrow[2] = {-INFINITY, -INFINITY}, lrow[2] = {0.f, 0.f};
+  const int irow[2] = {q0 + warp * 16 + g, q0 + warp * 16 + g + 8};
+
+  for (int k0 = 0; k0 < kv_len; k0 += AK) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < AK * (HD80 / 8); i += blockDim.x) {
+      const int r = i / (HD80 / 8), c = (i % (HD80 / 8)) * 8;
+      uint4 uk = make_uint4(0, 0, 0, 0), uv = make_uint4(0, 0, 0, 0);
+      if (k0 + r < kv_len) {
+        const long long row = (long long)b * p.kv_rows + p.kv_halo + k0 + r;
+        uk = *reinterpret_cast<const uint4*>(p.k + row * p.k_ld + h * HD80 + c);
+        uv = *reinterpret_cast<const uint4*>(p.v + row * p.v_ld + h * HD80 + c);
+      }
+      *reinterpret_cast<uint4*>(sK + r * LDS80 + c) = uk;
+      *reinterpret_cast<uint4*>(sV + r * LDS80 + c) = uv;
+    }
+    __syncthreads();
+    // S = Q K^T  (16 x 64 per warp)
+    float s[8][4];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
+#pragma unroll
+    for (int nt2 = 0; nt2 < 4; ++nt2) {
+#pragma unroll
+      for (int ks = 0; ks < 5; ++ks) {
+        uint32_t b0, b1, b2, b3;
+        const elem_t* ptr = sK + (nt2 * 16 + (lane & 7) + 8 * (lane >> 4)) * LDS80 + ks * 16 + 8 * ((lane >> 3) & 1);
+        ldsm_x4(b0, b1, b2, b3, ptr);
+        mma16816(s[2 * nt2], qa[ks], b0, b1);
+        mma16816(s[2 * nt2 + 1], qa[ks], b2, b3);
+      }
+    }
+    float mnew[2] = {mrow[0], mrow[1]};
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int j = k0 + nt * 8 + 2 * tq + (e & 1);
+        const float val = j >= kv_len ? -INFINITY : s[nt][e] * scale;
+        s[nt][e] = val;
+        mnew[e >> 1] = fmaxf(mnew[e >> 1], val);
+      }
+    }
+    float corr[2], msafe[2];
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      mnew[rr] = fmaxf(mnew[rr], __shfl_xor_sync(0xffffffffu, mnew[rr], 1));
+      mnew[rr] = fmaxf(mnew[rr], __shfl_xor_sync(0xffffffffu, mnew[rr], 2));
+      msafe[rr] = (mnew[rr] == -INFINITY) ? 0.f : mnew[rr];
+      corr[rr] = (mrow[rr] == -INFINITY) ? 0.f : __expf(mrow[rr] - msafe[rr]);
+      mrow[rr] = mnew[rr];
+      lrow[rr] *= corr[rr];
+    }
+#pragma unroll
+    for (int nt = 0; nt < 10; ++nt) {
+      o[nt][0] *= corr[0]; o[nt][1] *= corr[0]; o[nt][2] *= corr[1]; o[nt][3] *= corr[1];
+    }
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      const float p0 = __expf(s[nt][0] - msafe[0]), p1 = __expf(s[nt][1] - msafe[0]);
+      const float p2 = __expf(s[nt][2] - msafe[1]), p3 = __expf(s[nt][3] - msafe[1]);
+      lrow[0] += p0 + p1;
+      lrow[1] += p2 + p3;
+      const int ks = nt >> 1;
+      if ((nt & 1) == 0) { pa[ks][0] = pack_h2(p0, p1); pa[ks][1] = pack_h2(p2, p3); }
+      else               { pa[ks][2] = pack_h2(p0, p1); pa[ks][3] = pack_h2(p2, p3); }
+    }
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {      // 16 keys per k-step
+#pragma unroll
+      for (int nt2 = 0; nt2 < 5; ++nt2) { // 16 output dims per ldmatrix
+        uint32_t b0, b1, b2, b3;
+        const elem_t* ptr = sV + (ks * 16 + (lane & 7) + 8 * ((lane >> 3) & 1)) * LDS80 + nt2 * 16 + 8 * (lane >> 4);
+        ldsm_x4_t(b0, b1, b2, b3, ptr);
+        mma16816(o[2 * nt2], pa[ks], b0, b1);
+        mma16816(o[2 * nt2 + 1], pa[ks], b2, b3);
+      }
+    }
+  }
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    lrow[rr] += __shfl_xor_sync(0xffffffffu, lrow[rr], 1);
+    lrow[rr] += __shfl_xor_sync(0xffffffffu, lrow[rr], 2);
+  }
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    const int i = irow[rr];
+    if (i >= p.sq) continue;
+    const float inv = lrow[rr] > 0.f ? 1.f / lrow[rr] : 0.f;
+    elem_t* op = p.out + ((long long)b * p.q_rows + p.q_halo + i) * p.out_ld + h * HD80;
+#pragma unroll
+    for (int nt = 0; nt < 10; ++nt)
+      *reinterpret_cast<__half2*>(op + nt * 8 + 2 * tq) = __floats2half2_rn(o[nt][2 * rr] * inv, o[nt][2 * rr + 1] * inv);
+  }
+}
+
 }  // namespace sb
 
 extern "C" int sb_attention(const void* q, int64_t q_ld, const void* k, int64_t k_ld, const void* v, int64_t v_ld,
@@ -655,6 +785,26 @@ extern "C" int sb_attention_relpos(const void* q, int64_t q_ld, const void* k, i
   }
   dim3 grid((s + AQ - 1) / AQ, heads, batch);
   attention_kernel<true><<<grid, 128, smem, (cudaStream_t)stream>>>(a);
+  SB_LAUNCH_OK();
+  return SB_OK;
+}
+
+extern "C" int sb_attention_hd80(const void* q, int64_t q_ld, const void* k, int64_t k_ld, const void* v, int64_t v_ld, void* out,
+                                 int64_t out_ld, int32_t batch, int32_t heads, int32_t sq, int32_t sk, int32_t q_rows,
+                                 int32_t q_halo, int32_t kv_rows, int32_t kv_halo, const int32_t* kv_lens, sb_stream_t stream) {
+  using namespace sb;
+  SB_REQUIRE(q && k && v && out && batch > 0 && heads > 0 && sq > 0 && sk > 0, SB_EINVAL, "sb_attention_hd80: bad args");
+  SB_REQUIRE(batch <= 65535 && heads <= 65535, SB_EINVAL, "sb_attention_hd80: batch %d / heads %d exceed 65535", batch, heads);
+  SB_REQUIRE((q_ld % 8) == 0 && (k_ld % 8) == 0 && (v_ld % 8) == 0 && (out_ld % 2) == 0, SB_ENOSUP,
+             "sb_attention_hd80: row strides must be multiples of 8 elements");
+  AttnArgs a = {};
+  a.q = (const elem_t*)q; a.k = (const elem_t*)k; a.v = (const elem_t*)v; a.out = (elem_t*)out;
+  a.q_ld = q_ld; a.k_ld = k_ld; a.v_ld = v_ld; a.out_ld = out_ld;
+  a.batch = batch; a.heads = heads; a.sq = sq; a.sk = sk; a.q_rows = q_rows; a.q_halo = q_halo;
+  a.kv_rows = kv_rows; a.kv_halo = kv_halo; a.kv_lens = kv_lens;
+  const size_t smem = (size_t)(AQ + 2 * AK) * LDS80 * sizeof(elem_t);  // 33 KB
+  dim3 grid((sq + AQ - 1) / AQ, heads, batch);
+  attention_hd80_kernel<<<grid, 128, smem, (cudaStream_t)stream>>>(a);
   SB_LAUNCH_OK();
   return SB_OK;
 }

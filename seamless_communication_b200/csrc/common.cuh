@@ -91,12 +91,16 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
+// exact GELU (torch.nn.functional.gelu, approximate='none')
+__device__ __forceinline__ float gelu_erf(float v) { return 0.5f * v * (1.f + erff(v * 0.70710678118654752f)); }
+
 __device__ __forceinline__ float apply_act(float v, int act, float slope) {
   switch (act) {
     case SB_ACT_RELU: return fmaxf(v, 0.f);
     case SB_ACT_SILU: return v / (1.f + __expf(-v));
     case SB_ACT_LRELU: return v > 0.f ? v : v * slope;
     case SB_ACT_TANH: return tanhf(v);
+    case SB_ACT_GELU: return gelu_erf(v);
     default: return v;
   }
 }

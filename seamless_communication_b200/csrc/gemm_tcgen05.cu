@@ -51,6 +51,7 @@ struct GemmArgs {
   float2* tile_stats;    // optional [n tiles][m]: (max, sum exp(x - max)) of every output row over this CTA's BN columns
   const char* prefetch;  // weights of the kernel that follows: pulled into L2 by the idle epilogue warp during the main loop
   long long prefetch_bytes;
+  unsigned long long* argmin;  // sb_nearest_centroid: per row atomicMin of (orderable -2 v bits << 32 | column); no stores
 };
 
 template <int BN>
@@ -217,6 +218,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const bool has_res = valid && (g.res1 != nullptr || g.res2 != nullptr);
     const float post_scale = has_res ? g.gamma : g.alpha * g.gamma;
     float st_m = -INFINITY, st_s = 0.f;  // running log-sum-exp statistics of this thread's row (tile_stats)
+    unsigned long long best = ~0ull;      // argmin mode: this row's best (distance, column) over the tile
 #pragma unroll 1
     for (int c0 = 0; c0 < BN; c0 += 32) {
       if (n0 + c0 >= g.n) break;  // warp-uniform
@@ -250,6 +252,25 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       } else if (g.act == SB_ACT_TANH) {
 #pragma unroll
         for (int j = 0; j < 32; ++j) v[j] = tanhf(v[j]);
+      } else if (g.act == SB_ACT_GELU) {
+#pragma unroll
+        for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
+      }
+      if (g.argmin != nullptr) {
+        // v = x.c - |c|^2 / 2, so -2 v = |c|^2 - 2 x.c exactly (a power-of-two scale); the packed key orders by distance,
+        // then by column, and the running minimum over this row's chunks keeps the lowest column of equal distances
+        if (valid) {
+#pragma unroll
+          for (int j = 0; j < 32; ++j) {
+            if (oc + j < g.n) {
+              const unsigned int u = __float_as_uint(-2.f * v[j]);
+              const unsigned int key = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+              const unsigned long long pk = ((unsigned long long)key << 32) | (unsigned int)(oc + j);
+              best = pk < best ? pk : best;
+            }
+          }
+        }
+        continue;
       }
       const bool full = (oc + nv <= n_out_total);
       if (has_res) {
@@ -381,6 +402,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     }
     if (g.tile_stats != nullptr && row_ok) g.tile_stats[(long long)(n0 / BN) * g.m + m] = make_float2(st_m, st_s);
+    if (g.argmin != nullptr && best != ~0ull) atomicMin(g.argmin + m, best);
     if (g.tma_store) {
       // make the staged tile visible to the async proxy, then one thread issues the bulk tensor stores
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -472,6 +494,7 @@ static void fill_args(const sb_gemm_t* g, GemmArgs* a) {
   a->seq_rows = g->seq_rows; a->seq_halo = g->seq_halo; a->seq_len = g->seq_len; a->seq_lens = g->seq_lens;
   a->tile_stats = (float2*)g->tile_stats;
   a->prefetch = (const char*)g->prefetch; a->prefetch_bytes = g->prefetch ? g->prefetch_bytes / 4096 * 4096 : 0;
+  a->argmin = nullptr;
   a->tma_store = 0;
   a->kb_per_split = 0;
   a->slice_rows = 0;
@@ -479,7 +502,8 @@ static void fill_args(const sb_gemm_t* g, GemmArgs* a) {
 }
 
 template <int BN>
-static int launch(const sb_gemm_t* g, cudaStream_t st, int splits = 1, long long slice_rows = 0) {
+static int launch(const sb_gemm_t* g, cudaStream_t st, int splits = 1, long long slice_rows = 0,
+                  unsigned long long* argmin = nullptr) {
   using Cfg = TileCfg<BN>;
   static bool configured = false;
   if (!configured) {
@@ -503,6 +527,8 @@ static int launch(const sb_gemm_t* g, cudaStream_t st, int splits = 1, long long
   static int force_direct = -1;
   if (force_direct < 0) { const char* e = getenv("SB_GEMM_DIRECT_STORE"); force_direct = e ? atoi(e) : 0; }
   if (force_direct) tma_ok = false;
+  args.argmin = argmin;
+  if (argmin != nullptr) tma_ok = false;  // nothing is stored
   int kb_per = 0;
   if (splits > 1) {
     const int kb_total = g->taps * ((g->c_in + BK - 1) / BK);
@@ -636,6 +662,40 @@ extern "C" int sb_gemm_splitk(const sb_gemm_t* g_in, int32_t splits, float* part
   SB_REQUIRE(slice_rows >= g.m, SB_EINVAL, "sb_gemm_splitk: slice_rows (%lld) < m (%d)", (long long)slice_rows, g.m);
   // 64-wide tiles: twice the CTAs and half the (fp32) epilogue per CTA - these problems are latency bound
   return sb::launch<64>(&g, (cudaStream_t)stream, splits, slice_rows);
+}
+
+static __global__ void argmin_fill_kernel(unsigned long long* best, int rows) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r < rows) best[r] = ~0ull;
+}
+
+static __global__ void argmin_finish_kernel(const unsigned long long* best, int rows, int32_t* units) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r < rows) units[r] = best[r] == ~0ull ? -1 : (int32_t)(best[r] & 0xffffffffull);
+}
+
+extern "C" int sb_nearest_centroid(const void* x, int64_t x_ld, int32_t rows, int32_t dim, const void* centroids,
+                                   const float* neg_half_norm, int32_t K, int32_t seq_rows, const int32_t* seq_lens,
+                                   uint64_t* best, int32_t* units, sb_stream_t stream) {
+  SB_REQUIRE(x && centroids && neg_half_norm && best && units && rows > 0 && K > 0 && dim > 0, SB_EINVAL,
+             "sb_nearest_centroid: bad args");
+  SB_REQUIRE(seq_rows == 0 || seq_lens != nullptr, SB_EINVAL, "sb_nearest_centroid: seq_rows needs seq_lens");
+  sb_gemm_t g = {};
+  g.a = x; g.a_rows = rows; g.a_ld = x_ld; g.c_in = dim; g.taps = 1; g.dil = 1; g.a_row0 = 0;
+  g.w = centroids; g.n = K; g.m = rows; g.bias = neg_half_norm; g.act = SB_ACT_NONE; g.alpha = 1.f; g.gamma = 1.f;
+  g.out = best; g.out_ld = K;
+  g.seq_rows = seq_rows; g.seq_halo = 0; g.seq_len = 0; g.seq_lens = seq_lens;
+  int rc = sb::validate(&g);
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const unsigned blocks = (unsigned)((rows + 255) / 256);
+  argmin_fill_kernel<<<blocks, 256, 0, st>>>((unsigned long long*)best, rows);
+  SB_LAUNCH_OK();
+  rc = sb::launch<128>(&g, st, 1, 0, (unsigned long long*)best);
+  if (rc) return rc;
+  argmin_finish_kernel<<<blocks, 256, 0, st>>>((const unsigned long long*)best, rows, units);
+  SB_LAUNCH_OK();
+  return SB_OK;
 }
 
 extern "C" int sb_gemm_debug_timeline(unsigned long long* buf) {

@@ -6,6 +6,8 @@ namespace sb {
 
 constexpr int LN_MAX_CHUNKS = 8;  // dim <= 8 * 256 = 2048
 
+// ACT: SB_ACT_NONE (sb_layernorm) or SB_ACT_GELU (sb_layernorm_gelu, applied before the fp16 rounding)
+template <int ACT>
 __global__ void __launch_bounds__(256) layernorm_kernel(const elem_t* __restrict__ x, const elem_t* __restrict__ res,
                                                         elem_t* __restrict__ y, elem_t* __restrict__ sum_out,
                                                         const float* __restrict__ w, const float* __restrict__ bvec, int dim,
@@ -90,6 +92,10 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const elem_t* __restrict
       for (int e = 0; e < 4; ++e) {
         float a0 = masked ? 0.f : (v[c][2 * e] - mean) * rstd * ww[2 * e] + bb[2 * e];
         float a1 = masked ? 0.f : (v[c][2 * e + 1] - mean) * rstd * ww[2 * e + 1] + bb[2 * e + 1];
+        if constexpr (ACT == SB_ACT_GELU) {
+          a0 = gelu_erf(a0);
+          a1 = gelu_erf(a1);
+        }
         ho[e] = __floats2half2_rn(a0, a1);
       }
       *reinterpret_cast<uint4*>(yp + off) = o;
@@ -227,9 +233,24 @@ extern "C" int sb_layernorm(const void* x, const void* res, void* y, void* sum_o
   SB_REQUIRE(dim % 8 == 0 && dim <= 256 * LN_MAX_CHUNKS, SB_ENOSUP, "sb_layernorm: dim %d unsupported (multiple of 8, <= 2048)", dim);
   const long long rows = (long long)batch * T;
   const int wpb = rows >= 4096 ? 8 : 2;  // small problems: more CTAs, shorter critical path
-  SB_CUDA_OK(launch_k(layernorm_kernel, dim3((unsigned)((rows + wpb - 1) / wpb)), dim3(wpb * 32), 0, (cudaStream_t)stream,
+  SB_CUDA_OK(launch_k(layernorm_kernel<SB_ACT_NONE>, dim3((unsigned)((rows + wpb - 1) / wpb)), dim3(wpb * 32), 0, (cudaStream_t)stream,
                        (const elem_t*)x, (const elem_t*)res, (elem_t*)y, (elem_t*)sum_out, w, b, (int)dim, rows, (int)T,
                        (int)in_rows, (int)in_halo, (int)out_rows, (int)out_halo, lens, (int)mask_out));
+  count_launch();
+  return SB_OK;
+}
+
+extern "C" int sb_layernorm_gelu(const void* x, void* y, const float* w, const float* b, int32_t dim, int32_t batch, int32_t T,
+                                 int32_t in_rows, int32_t in_halo, int32_t out_rows, int32_t out_halo, const int32_t* lens,
+                                 int32_t mask_out, sb_stream_t stream) {
+  using namespace sb;
+  SB_REQUIRE(x && y && w && b && batch > 0 && T > 0, SB_EINVAL, "sb_layernorm_gelu: bad args");
+  SB_REQUIRE(dim % 8 == 0 && dim <= 256 * LN_MAX_CHUNKS, SB_ENOSUP, "sb_layernorm_gelu: dim %d unsupported (multiple of 8, <= 2048)", dim);
+  const long long rows = (long long)batch * T;
+  const int wpb = rows >= 4096 ? 8 : 2;
+  SB_CUDA_OK(launch_k(layernorm_kernel<SB_ACT_GELU>, dim3((unsigned)((rows + wpb - 1) / wpb)), dim3(wpb * 32), 0,
+                       (cudaStream_t)stream, (const elem_t*)x, (const elem_t*)nullptr, (elem_t*)y, (elem_t*)nullptr, w, b,
+                       (int)dim, rows, (int)T, (int)in_rows, (int)in_halo, (int)out_rows, (int)out_halo, lens, (int)mask_out));
   count_launch();
   return SB_OK;
 }

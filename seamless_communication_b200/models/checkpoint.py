@@ -177,5 +177,37 @@ def convert_vocoder_checkpoint(checkpoint: Mapping[str, Any]) -> Dict[str, Any]:
     return out
 
 
+_W2V2_RULES = [(re.compile(a), b) for a, b in (
+    # frontend, as the reference's conformer_shaw/loader.py:44-70 maps a fairseq wav2vec2 model
+    (r"^encoder\.pos_conv\.0\.", "encoder_frontend.pos_encoder.conv."),
+    (r"^feature_extractor\.conv_layers\.([0-9]+)\.0\.", r"encoder_frontend.feature_extractor.layers.\1.conv."),
+    (r"^feature_extractor\.conv_layers\.([0-9]+)\.2\.1\.", r"encoder_frontend.feature_extractor.layers.\1.layer_norm."),
+    (r"^layer_norm\.", "encoder_frontend.post_extract_layer_norm."),
+    (r"^post_extract_proj\.", "encoder_frontend.model_dim_proj."),
+    # plain pre-LN Transformer layers (fairseq2's wav2vec2 loader; recalled, DESIGN.md section 11)
+    (r"^encoder\.layers\.([0-9]+)\.self_attn\.out_proj\.", r"encoder.layers.\1.self_attn.output_proj."),
+    (r"^encoder\.layers\.([0-9]+)\.fc1\.", r"encoder.layers.\1.ffn.inner_proj."),
+    (r"^encoder\.layers\.([0-9]+)\.fc2\.", r"encoder.layers.\1.ffn.output_proj."),
+    (r"^encoder\.layers\.([0-9]+)\.final_layer_norm\.", r"encoder.layers.\1.ffn_layer_norm."),
+)]
+
+
+def convert_wav2vec2_checkpoint(checkpoint: Mapping[str, Any]) -> Dict[str, Any]:
+    """fairseq `xlsr2_1b_v2.pt` ({"model": fairseq names}) -> {"model": fairseq2 names}.  Keys no rule matches keep their
+    name (self_attn.{q,k,v}_proj, self_attn_layer_norm and encoder.layer_norm are spelled alike in both); a dict already
+    in fairseq2 names passes through unchanged."""
+    sd = checkpoint.get("model", checkpoint)
+    if any(k.startswith("encoder_frontend.") for k in sd):
+        return {"model": dict(sd)}
+    out: Dict[str, Any] = {}
+    for k, v in sd.items():
+        for pat, rep in _W2V2_RULES:
+            if pat.search(k):
+                k = pat.sub(rep, k)
+                break
+        out[k] = v
+    return {"model": out}
+
+
 def load_checkpoint_file(path: str) -> Dict[str, Any]:
     return torch.load(path, map_location="cpu", weights_only=True)

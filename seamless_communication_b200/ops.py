@@ -10,7 +10,7 @@ import torch
 from . import _lib
 from ._lib import BeamDesc, GemmDesc, check
 
-ACT_NONE, ACT_RELU, ACT_SILU, ACT_LRELU, ACT_TANH = 0, 1, 2, 3, 4
+ACT_NONE, ACT_RELU, ACT_SILU, ACT_LRELU, ACT_TANH, ACT_GELU = 0, 1, 2, 3, 4, 5
 F16 = torch.float16
 
 
@@ -275,6 +275,77 @@ def fbank(wave: torch.Tensor, num_samples: torch.Tensor, frames_ld: int, standar
     check(lib.sb_fbank(wave.data_ptr(), wave.stride(0), num_samples.data_ptr(), B, out.data_ptr(), frames_ld,
                        work.data_ptr(), frames.data_ptr(), int(standardize), _stream()), "sb_fbank")
     return out, frames
+
+
+def w2v2_front(wave: torch.Tensor, num_samples: torch.Tensor, w0, b0, ln_w, ln_b, out_rows: int) -> Seq:
+    """wave (B, T) fp32 cuda, num_samples (B,) int32 cuda -> feature-extractor layer 0 output, (B, out_rows, 512) fp16
+    with frames past each row's count written as 0 (sb_w2v2_front)."""
+    lib = _lib.load()
+    B = wave.shape[0]
+    out = Seq(B, out_rows, 512, zero=False)
+    stats = torch.empty((B, 2), dtype=torch.float32, device=wave.device)
+    check(lib.sb_w2v2_front(wave.data_ptr(), wave.stride(0), num_samples.data_ptr(), B, w0.data_ptr(), b0.data_ptr(),
+                            ln_w.data_ptr(), ln_b.data_ptr(), out.buf.data_ptr(), out_rows, stats.data_ptr(), _stream()),
+          "sb_w2v2_front")
+    return out
+
+
+def layernorm_gelu(x: Seq, w, b, *, out: Optional[Seq] = None, mask=True) -> Seq:
+    """GELU(LayerNorm(x)) per row (sb_layernorm_gelu); with x.lens and mask, rows past each length are written as 0."""
+    lib = _lib.load()
+    if out is None:
+        out = x.like(zero=x.PH > 0 or x.Tp != x.T)
+    assert x.buf.stride(0) == x.C and out.buf.stride(0) == x.C
+    check(lib.sb_layernorm_gelu(x.buf.data_ptr(), out.buf.data_ptr(), w.data_ptr(), b.data_ptr(), x.C, x.B, x.T, x.Tp, x.PH,
+                                out.Tp, out.PH, _p(x.lens), int(mask and x.lens is not None), _stream()), "sb_layernorm_gelu")
+    return out
+
+
+def attention_hd80(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tensor, B, H, sq, sk, q_rows, q_halo,
+                   kv_rows, kv_halo, kv_lens=None):
+    """sb_attention's contract at head_dim 80 (scale 80^-0.5, key mask only)."""
+    lib = _lib.load()
+    check(lib.sb_attention_hd80(q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0),
+                                out.data_ptr(), out.stride(0), B, H, sq, sk, q_rows, q_halo, kv_rows, kv_halo, _p(kv_lens),
+                                _stream()), "sb_attention_hd80")
+    return out
+
+
+def grouped_conv_gelu_res(x: Seq, ws, bias, taps: int, out: Seq) -> Seq:
+    """out = x + GELU(Conv1d(x)) for a grouped 'same' conv with an even kernel whose last output frame is dropped
+    (wav2vec2's positional conv): output row t reads input rows t - taps/2 .. t + taps/2 - 1.  ws: one (C/G, taps*C/G)
+    packed weight per group; x is dense (PH = 0) and every sequence is followed by at least taps/2 zero rows, which are
+    the conv's zero padding on both sides of its neighbours (rows before the buffer read as zero).  One sb_gemm per group;
+    every row of out is written."""
+    lib = _lib.load()
+    assert x.PH == 0 and out.PH == 0 and out.Tp == x.Tp and x.buf.stride(0) == x.C
+    G = len(ws)
+    cg = x.C // G
+    esz = x.buf.element_size()
+    for g in range(G):
+        d = GemmDesc()
+        d.a, d.a_rows, d.a_ld, d.c_in, d.taps, d.dil = x.buf.data_ptr() + g * cg * esz, x.B * x.Tp, x.C, cg, taps, 1
+        d.a_row0 = -(taps // 2)
+        d.w, d.n, d.m = ws[g].data_ptr(), cg, x.B * x.Tp
+        d.bias, d.act, d.alpha, d.gamma = bias.data_ptr() + g * cg * 4, ACT_GELU, 1.0, 1.0
+        d.res1, d.res1_ld = x.buf.data_ptr() + g * cg * esz, x.C
+        d.out, d.out_ld = out.buf.data_ptr() + g * cg * esz, out.buf.stride(0)
+        check(lib.sb_gemm(C.byref(d), _stream()), "sb_gemm")
+    return out
+
+
+def nearest_centroid(x: Seq, centroids: torch.Tensor, neg_half_norm: torch.Tensor, lens: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """units (B*Tp,) int32: per row the index of the nearest centroid (ties to the lowest), -1 on rows at or past
+    lens[b] (sb_nearest_centroid)."""
+    lib = _lib.load()
+    assert x.PH == 0
+    rows = x.B * x.Tp
+    best = torch.empty((rows,), dtype=torch.int64, device=x.buf.device)
+    units = torch.empty((rows,), dtype=torch.int32, device=x.buf.device)
+    check(lib.sb_nearest_centroid(x.buf.data_ptr(), x.buf.stride(0), rows, x.C, centroids.data_ptr(), neg_half_norm.data_ptr(),
+                                  centroids.shape[0], x.Tp if lens is not None else 0, _p(lens), best.data_ptr(),
+                                  units.data_ptr(), _stream()), "sb_nearest_centroid")
+    return units
 
 
 def embed_seq(ids: torch.Tensor, embed, pos, scale, dim) -> torch.Tensor:

@@ -23,7 +23,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 
-from .config import UnitYConfig, VocoderConfig
+from .config import UnitYConfig, VocoderConfig, Wav2Vec2EncoderConfig
 
 SPACE = "▁"
 
@@ -456,3 +456,42 @@ def make_monotonic_state_dict(cfg: UnitYConfig, seed: int = 2, logit_scale: floa
         I.sd[f"{p}.energy_bias"] = torch.full((1,), energy_bias)
     sd.update(I.sd)
     return sd
+
+
+def make_wav2vec2_state_dict(cfg: Wav2Vec2EncoderConfig, seed: int = 3) -> Dict[str, torch.Tensor]:
+    """Random-init wav2vec2 encoder weights under fairseq2's names (the names `convert_wav2vec2_checkpoint` produces),
+    with the other synthetic models' init scale; the positional conv keeps its weight-norm pair (weight_g, weight_v)."""
+    I = _Init(seed)
+    M, F = cfg.model_dim, cfg.feature_dim
+    c_in = 1
+    for i, (c, k, _) in enumerate(cfg.feature_extractor_layer_descs):
+        p = f"encoder_frontend.feature_extractor.layers.{i}"
+        I.conv(p + ".conv", c, c_in, k)
+        I.ln(p + ".layer_norm", c)
+        c_in = c
+    I.ln("encoder_frontend.post_extract_layer_norm", F)
+    I.linear("encoder_frontend.model_dim_proj", M, F)
+    K, G = cfg.pos_conv_kernel_size, cfg.num_pos_conv_groups
+    p = "encoder_frontend.pos_encoder.conv"
+    I.normal(p + ".weight_v", (M, M // G, K), 1.0 / math.sqrt(M // G * K))
+    v = I.sd[p + ".weight_v"].double()
+    # weight_g starts at the norm of weight_v per tap (what weight_norm's init gives), scaled so the fold is not a no-op
+    I.sd[p + ".weight_g"] = _round_fp16((v.pow(2).sum((0, 1)).sqrt() * (1.0 + 0.1 * torch.randn(K, generator=I.g).double()))
+                                        .float().reshape(1, 1, K))
+    I.normal(p + ".bias", (M,), 0.02)
+    for i in range(cfg.num_encoder_layers):
+        p = f"encoder.layers.{i}"
+        I.ln(p + ".self_attn_layer_norm", M)
+        for q in ("q_proj", "k_proj", "v_proj", "output_proj"):
+            I.linear(f"{p}.self_attn.{q}", M, M)
+        I.ln(p + ".ffn_layer_norm", M)
+        I.linear(p + ".ffn.inner_proj", cfg.ffn_inner_dim, M)
+        I.linear(p + ".ffn.output_proj", M, cfg.ffn_inner_dim)
+    I.ln("encoder.layer_norm", M)
+    return I.sd
+
+
+def make_kmeans_centroids(num: int, dim: int, seed: int = 4, scale: float = 1.0) -> torch.Tensor:
+    """(num, dim) fp32 centroids on the fp16 grid (the layout KmeansModel's `.npy` is transposed to, kmeans.py:17-19)."""
+    g = torch.Generator().manual_seed(seed)
+    return _round_fp16(torch.randn(num, dim, generator=g) * scale)
