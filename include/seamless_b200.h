@@ -46,6 +46,8 @@ int64_t sb_launch_count(void);
  *   out[q, n] = gamma * (alpha * v + res1[q, n] + res2[q, n]),  q = m + out_row0
  *   out2[q, n] = leaky_relu(out[q, n], out2_slope)                         (optional second output)
  *   rows q whose sequence position is outside [0, len) are written as zeros (when seq_rows > 0).
+ * SB_EINVAL unless a, w, out and (when set) out2, res1, res2 are 16-byte aligned, m <= 65535 * 128, and out_f32 = 1
+ * whenever tile_stats is set.
  * Replaces: fairseq2 Linear / torch Conv1d / ConvTranspose1d call sites of the path, e.g. Linear_forward
  * (ggml/examples/unity/fairseq2.cpp:251), ggml_conv_1d in ConvModule_forward (fairseq2.cpp:698-731),
  * Conv1dBlock.forward (models/unity/fft_decoder_layer.py:75-101), hifigan.py:114-121,180-196.
@@ -78,7 +80,8 @@ typedef struct {
   const void* prefetch;    /* optional: a device range (e.g. the next layer's weights) to pull into L2 while this GEMM runs */
   int64_t prefetch_bytes;
   float* tile_stats;       /* optional fp32 [ceil(n/128)][m][2]: per output row and 128-column tile (max, sum exp(x - max)) of
-                              the stored values - log-softmax statistics fused into the projection (sb_logits_topk_tiles) */
+                              the stored fp32 values (needs out_f32) - log-softmax statistics fused into the projection
+                              (sb_logits_topk_tiles) */
 } sb_gemm_t;
 
 int sb_gemm(const sb_gemm_t* g, sb_stream_t stream);

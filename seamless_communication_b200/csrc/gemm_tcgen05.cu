@@ -479,6 +479,11 @@ static int validate(const sb_gemm_t* g) {
   SB_REQUIRE((g->a_ld % 8) == 0 && (g->c_in % 8) == 0, SB_ENOSUP, "sb_gemm: a_ld (%lld) and c_in (%d) must be multiples of 8",
              (long long)g->a_ld, g->c_in);
   SB_REQUIRE(((uintptr_t)g->a % 16) == 0 && ((uintptr_t)g->w % 16) == 0, SB_EINVAL, "sb_gemm: operands must be 16B aligned");
+  // the direct-store epilogue's 16-byte residual loads and output stores check only ld and the column for alignment
+  SB_REQUIRE(((uintptr_t)g->out % 16) == 0 && ((uintptr_t)g->out2 % 16) == 0 && ((uintptr_t)g->res1 % 16) == 0 &&
+                 ((uintptr_t)g->res2 % 16) == 0,
+             SB_EINVAL, "sb_gemm: out, out2, res1 and res2 must be 16B aligned");
+  SB_REQUIRE(g->m <= 65535 * BM, SB_EINVAL, "sb_gemm: m (%d) exceeds %d rows (65535 row tiles)", g->m, 65535 * BM);
   SB_REQUIRE(!g->glu || (g->n % 2) == 0, SB_EINVAL, "sb_gemm: glu needs even n");
   return SB_OK;
 }
@@ -517,13 +522,18 @@ static int launch(const sb_gemm_t* g, cudaStream_t st, int splits = 1, long long
   if (rc) return rc;
   GemmArgs args;
   fill_args(g, &args);
-  // staged TMA-store epilogue needs 128 B output groups (64 fp16 / 32 fp32 columns) and 16 B aligned rows
+  // staged TMA-store epilogue needs 128 B output groups (64 fp16 / 32 fp32 columns) and 16 B aligned rows.  The bulk
+  // store writes a row's last 16-byte unit whole, so a row that ends inside one (n_out * esize not a multiple of 16)
+  // would also overwrite the caller's columns after n_out: such outputs take the direct store.
   const int esize = g->out_f32 ? 4 : 2;
   const int n_tile_out = g->glu ? BN / 2 : BN;
   const int n_out_total = g->glu ? g->n / 2 : g->n;
   bool tma_ok = n_tile_out * esize >= 128 && ((uintptr_t)g->out % 16) == 0 && ((g->out_ld * esize) % 16) == 0 &&
-                g->out_row0 >= 0 && (g->out_row0 + g->m) < (1ll << 31) && !(g->glu && g->out_f32);
-  if (g->out2 != nullptr) tma_ok = tma_ok && ((uintptr_t)g->out2 % 16) == 0 && ((g->out2_ld * 2) % 16) == 0 && n_tile_out >= 64;
+                (n_out_total * esize) % 16 == 0 && g->out_row0 >= 0 && (g->out_row0 + g->m) < (1ll << 31) &&
+                !(g->glu && g->out_f32);
+  if (g->out2 != nullptr)
+    tma_ok = tma_ok && ((uintptr_t)g->out2 % 16) == 0 && ((g->out2_ld * 2) % 16) == 0 && (n_out_total * 2) % 16 == 0 &&
+             n_tile_out >= 64;
   static int force_direct = -1;
   if (force_direct < 0) { const char* e = getenv("SB_GEMM_DIRECT_STORE"); force_direct = e ? atoi(e) : 0; }
   if (force_direct) tma_ok = false;
@@ -618,20 +628,25 @@ extern "C" int sb_gemm(const sb_gemm_t* g_in, sb_stream_t stream) {
   cudaStream_t st = (cudaStream_t)stream;
   // Narrow-channel undilated convs (HiFi-GAN stages with C = 16/32): the taps of an output row are `taps` consecutive
   // input rows, i.e. one contiguous run of taps*C elements when rows are dense.  Describing A as overlapping rows of
-  // that length (row pitch still C) turns `taps` nearly empty 64-deep k-blocks into ceil(taps*C/64) full ones.
+  // that length (row pitch still C) turns `taps` nearly empty 64-deep k-blocks into ceil(taps*C/64) full ones.  TMA
+  // zero-fills such a window as a whole, so the collapse applies only when every window lies inside [0, a_rows): a
+  // window that starts before row 0 or runs past a_rows keeps the per-tap path, which zero-fills just its outside taps.
   sb_gemm_t gc;
   const sb_gemm_t* g = g_in;
-  if (g_in->taps > 1 && g_in->dil == 1 && g_in->c_in < sb::BK && g_in->a_ld == g_in->c_in) {
+  if (g_in->taps > 1 && g_in->dil == 1 && g_in->c_in < sb::BK && g_in->a_ld == g_in->c_in && g_in->a_row0 >= 0 &&
+      (long long)g_in->a_row0 + g_in->m + g_in->taps - 1 <= g_in->a_rows) {
     gc = *g_in;
     gc.c_in = g_in->taps * g_in->c_in;
     gc.taps = 1;
-    gc.a_rows = g_in->a_rows - (g_in->taps - 1);  // windows starting later would run past the buffer: zero-filled instead
+    gc.a_rows = g_in->a_rows - (g_in->taps - 1);
     g = &gc;
   }
   const long long mt = (g->m + sb::BM - 1) / sb::BM;
   const int sms = sb::sm_count();
   auto tiles = [&](int bn) { return mt * ((g->n + bn - 1) / bn); };
   if (g->tile_stats != nullptr) {
+    // the statistics are taken of the fp32 values the epilogue stores; an fp16 output would round after them
+    SB_REQUIRE(g->out_f32, SB_EINVAL, "sb_gemm: tile_stats needs out_f32");
     SB_REQUIRE(!g->glu && g->n >= 128, SB_ENOSUP, "sb_gemm: tile_stats needs n >= 128 and no GLU");
     // up to 256 rows (a beam-search step): the weight-stationary kernel of decode_gemm.cu, which reads each weight row once.
     // SB_PROJ_T=0 selects the general kernel (read per call: tools compare both inside one process)
