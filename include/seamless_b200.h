@@ -38,6 +38,8 @@ const char* sb_last_error(void);
 int sb_version(void);
 /* number of kernels launched by this library since load (bench.py reports it as gpu_launches) */
 int64_t sb_launch_count(void);
+/* 1 when kernels launch with programmatic dependent launch (the default; SB_PDL=0 in the environment turns it off) */
+int sb_pdl_enabled(void);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * sb_gemm - fused Linear / Conv1d-as-GEMM on Hopper tensor cores (TMA -> smem -> wgmma -> registers -> epilogue).

@@ -53,6 +53,7 @@ PROTOTYPES = {
     "sb_last_error": [],
     "sb_version": [],
     "sb_launch_count": [],
+    "sb_pdl_enabled": [],
     "sb_gemm": [C.POINTER(GemmDesc), c_p],
     "sb_gemm_ref": [C.POINTER(GemmDesc), c_p],
     "sb_gemm_splitk": [C.POINTER(GemmDesc), i32, c_p, i64, c_p],

@@ -46,11 +46,19 @@ inline void count_launch(int n = 1) { __atomic_fetch_add(&g_launch_count, (long 
     sb::count_launch();                                                                  \
   } while (0)
 
-// Programmatic dependent launch (PDL, opt-in with SB_PDL=1): every kernel waits for its prerequisites right before it
-// first touches data produced upstream and only THEN lets its own dependents launch, so launch latency, prologues
-// (barrier init, descriptor fetch) and - in the GEMMs - the weight loads of kernel N+1 overlap with
+// Programmatic dependent launch (PDL, on by default; SB_PDL=0 turns it off): every kernel waits for its prerequisites
+// right before it first touches data produced upstream and only THEN lets its own dependents launch, so launch latency,
+// prologues (barrier init, descriptor fetch) and - in the GEMMs - the weight loads of kernel N+1 overlap with
 // kernel N, while at most one generation of dependents is resident.  (Triggering at kernel entry instead would let the
 // whole chain launch ahead, with every waiting kernel pinning shared memory.)
+// The rule every kernel launched through launch_k keeps: each CTA runs pdl_wait (griddepcontrol.wait) before
+//   (a) it reads anything an earlier kernel wrote,
+//   (b) it writes global memory that an earlier kernel reads or writes, and
+//   (c) it exits.
+// Before the wait a CTA may only touch what no kernel of the stream writes (weights, biases, tensor maps) and its own
+// shared memory.  (c) keeps the chain transitive: the wait covers only the immediate predecessor, so a CTA that exited
+// early would let its grid complete - and its dependent pass the wait - while the kernel before it still runs.  Threads of
+// a CTA that exit without waiting (a producer lane, an idle warp) are fine as long as another thread of the CTA waits.
 // Both instructions are no-ops when the kernel was launched without the attribute.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -64,6 +72,17 @@ int make_tmap(CUtensorMap* tm, const void* base, uint64_t inner, uint64_t rows, 
 // sb_gemm with tile_stats at <= 256 rows on the weight-stationary projection kernel (decode_gemm.cu).  Returns false,
 // launching nothing, when the shape does not qualify; else true with the launch's status in *rc.
 bool vocab_proj(const sb_gemm_t* g, cudaStream_t st, int* rc);
+
+// The beam-search step's small kernels (embedding, LayerNorms, attention, top-K, bookkeeping) ask for the largest shared
+// memory carveout of the SM's unified L1 / shared memory.  Under PDL the weight product that follows one of them
+// launches while it runs, and its CTAs (110-221 KB of shared memory) can only start on an SM whose carveout already
+// holds them; at the small default carveout such kernels leave, they wait for the SM to drain.  Measured on an H100 SXM
+// at 700 W: one search step 2.19 ms against 2.25 ms with PDL alone.  Without PDL nothing overlaps and the hint is not set.
+template <typename... KArgs>
+inline cudaError_t prefer_shared(void (*kernel)(KArgs...)) {
+  if (!pdl_enabled()) return cudaSuccess;
+  return cudaFuncSetAttribute((const void*)kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+}
 
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {

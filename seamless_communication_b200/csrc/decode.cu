@@ -942,6 +942,7 @@ extern "C" int sb_embed_step(const int32_t* seqs, int32_t seq_ld, const int32_t*
                              const void* pos_table, float scale, void* x, int32_t rows, int32_t dim, sb_stream_t stream) {
   using namespace sb;
   SB_REQUIRE(seqs && step_ptr && embed && pos_table && x && rows > 0 && dim % 2 == 0, SB_EINVAL, "sb_embed_step: bad args");
+  SB_CUDA_OK(prefer_shared(embed_kernel));
   SB_CUDA_OK(launch_k(embed_kernel, dim3(rows, 1), dim3(128), 0, (cudaStream_t)stream, (const int*)seqs, (long long)seq_ld,
                        (const int*)step_ptr, 1, (const elem_t*)embed, (const float*)pos_table, scale, (elem_t*)x, (int)dim));
   count_launch();
@@ -980,6 +981,7 @@ extern "C" int sb_decode_self_attn(const void* qkv, const float* qkv_partials, i
   if (v2 < 0) { const char* e = getenv("SB_SELF_ATTN_V2"); v2 = (e == nullptr || atoi(e) != 0) ? 1 : 0; }
   if (v2 && qkv == nullptr && (size_t)4 * max_len * sizeof(int) <= 48 * 1024) {
     if (max_len > 2048) SB_CUDA_OK(allow_dynamic_smem(decode_self_attn2_kernel, (size_t)4 * max_len * sizeof(int)));
+    SB_CUDA_OK(prefer_shared(decode_self_attn2_kernel));
     SB_CUDA_OK(launch_k(decode_self_attn2_kernel, dim3(rows, (heads + 3) / 4), dim3(128), (size_t)4 * max_len * sizeof(int),
                          (cudaStream_t)stream, qkv_partials, (int)splits, (long long)slice_rows, qkv_bias, (elem_t*)kcache, (elem_t*)vcache,
                          (const int*)anc, (int)anc_ld, (const int*)step_ptr, (int)max_len, (elem_t*)out, (int)rows, (int)heads));
@@ -989,6 +991,7 @@ extern "C" int sb_decode_self_attn(const void* qkv, const float* qkv_partials, i
   size_t smem = (size_t)8 * max_len * sizeof(float);
   SB_REQUIRE(smem <= 48 * 1024, SB_ENOSUP, "sb_decode_self_attn: max_len %d too large", max_len);
   if (max_len > 1024) SB_CUDA_OK(allow_dynamic_smem(decode_self_attn_kernel, smem));
+  SB_CUDA_OK(prefer_shared(decode_self_attn_kernel));
   SB_CUDA_OK(launch_k(decode_self_attn_kernel, dim3(rows, (heads + 3) / 4), dim3(128), smem, (cudaStream_t)stream,
                        (const elem_t*)qkv, qkv_partials, (int)splits, (long long)slice_rows, qkv_bias, (elem_t*)kcache,
                        (elem_t*)vcache, (const int*)anc, (int)anc_ld, (const int*)step_ptr,
@@ -1014,6 +1017,7 @@ extern "C" int sb_decode_cross_attn(const void* q, const float* q_partials, int3
         SB_CUDA_OK(cudaFuncSetAttribute(decode_cross_attn_shared_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
         configured = sm;
       }
+      SB_CUDA_OK(prefer_shared(decode_cross_attn_shared_kernel));
       SB_CUDA_OK(launch_k(decode_cross_attn_shared_kernel, dim3(rows / beam, heads), dim3(nw * 32), sm, (cudaStream_t)stream, q_partials,
                            (int)splits, (long long)slice_rows, q_bias, (const elem_t*)k, (const elem_t*)v, (long long)kv_ld,
                            (const int*)enc_lens, (int)s_enc, (elem_t*)out, (int)beam, (int)heads));
@@ -1023,6 +1027,7 @@ extern "C" int sb_decode_cross_attn(const void* q, const float* q_partials, int3
   }
   size_t smem = (size_t)4 * s_enc * sizeof(float);
   SB_REQUIRE(smem <= 48 * 1024, SB_ENOSUP, "sb_decode_cross_attn: s_enc %d too large", s_enc);
+  SB_CUDA_OK(prefer_shared(decode_cross_attn_kernel));
   SB_CUDA_OK(launch_k(decode_cross_attn_kernel, dim3(rows, (heads + 3) / 4), dim3(128), smem, (cudaStream_t)stream,
                        (const elem_t*)q, q_partials, (int)splits, (long long)slice_rows, q_bias, (const elem_t*)k,
                        (const elem_t*)v, (long long)kv_ld, (const int*)enc_lens, (int)s_enc,
@@ -1037,6 +1042,7 @@ extern "C" int sb_logits_topk(const float* logits, int64_t ld, int32_t rows, int
   using namespace sb;
   SB_REQUIRE(logits && cand_val && cand_idx && eos_lprob && rows > 0 && vocab > 0, SB_EINVAL, "sb_logits_topk: bad args");
   SB_REQUIRE(K > 0 && K <= TK_MAX, SB_ENOSUP, "sb_logits_topk: K=%d unsupported (<= %d)", K, TK_MAX);
+  SB_CUDA_OK(prefer_shared((logits_topk_kernel<false>)));
   SB_CUDA_OK(launch_k(logits_topk_kernel<false>, dim3(rows), dim3(TK_THREADS), 0, (cudaStream_t)stream, logits, (long long)ld,
                        (int)vocab, (int)pad_idx, (int)eos_idx, (int)unk_idx, unk_penalty, (int)K, cand_val, (int*)cand_idx,
                        eos_lprob, (const int*)nullptr, (const int*)nullptr, 0));
@@ -1055,6 +1061,7 @@ extern "C" int sb_logits_topk_ban(const float* logits, int64_t ld, int32_t rows,
   const size_t smem = (size_t)(vocab + 31) / 32 * sizeof(unsigned);
   SB_REQUIRE(smem <= 160 * 1024, SB_ENOSUP, "sb_logits_topk_ban: vocabulary of %d too large", vocab);
   SB_CUDA_OK(allow_dynamic_smem(logits_topk_kernel<true>, smem));
+  SB_CUDA_OK(prefer_shared((logits_topk_kernel<true>)));
   SB_CUDA_OK(launch_k(logits_topk_kernel<true>, dim3(rows), dim3(TK_THREADS), smem, (cudaStream_t)stream, logits, (long long)ld,
                        (int)vocab, (int)pad_idx, (int)eos_idx, (int)unk_idx, unk_penalty, (int)K, cand_val, (int*)cand_idx,
                        eos_lprob, (const int*)ban_ids, (const int*)ban_n, (int)ban_ld));
@@ -1072,6 +1079,7 @@ extern "C" int sb_logits_topk_tiles(const float* logits, int64_t ld, const float
   const int n_tiles = (vocab + TKT_TILE - 1) / TKT_TILE;
   const size_t smem = (size_t)2 * n_tiles * sizeof(float);
   SB_REQUIRE(smem <= 40 * 1024, SB_ENOSUP, "sb_logits_topk_tiles: vocabulary of %d too large", vocab);
+  SB_CUDA_OK(prefer_shared((logits_topk_tiles_kernel<false>)));
   SB_CUDA_OK(launch_k(logits_topk_tiles_kernel<false>, dim3(rows), dim3(TKT_THREADS), smem, (cudaStream_t)stream, logits, (long long)ld,
                        (const float2*)tile_stats, (int)rows, (int)vocab, (int)pad_idx, (int)eos_idx, (int)unk_idx, unk_penalty, (int)K,
                        cand_val, (int*)cand_idx, eos_lprob, (const int*)nullptr, (const int*)nullptr, 0));
@@ -1092,6 +1100,7 @@ extern "C" int sb_logits_topk_tiles_ban(const float* logits, int64_t ld, const f
   const size_t smem = (size_t)2 * n_tiles * sizeof(float) + (size_t)(vocab + 31) / 32 * sizeof(unsigned);
   SB_REQUIRE((size_t)2 * n_tiles * sizeof(float) <= 40 * 1024, SB_ENOSUP, "sb_logits_topk_tiles_ban: vocabulary of %d too large", vocab);
   SB_CUDA_OK(allow_dynamic_smem(logits_topk_tiles_kernel<true>, smem));
+  SB_CUDA_OK(prefer_shared((logits_topk_tiles_kernel<true>)));
   SB_CUDA_OK(launch_k(logits_topk_tiles_kernel<true>, dim3(rows), dim3(TKT_THREADS), smem, (cudaStream_t)stream, logits, (long long)ld,
                        (const float2*)tile_stats, (int)rows, (int)vocab, (int)pad_idx, (int)eos_idx, (int)unk_idx, unk_penalty, (int)K,
                        cand_val, (int*)cand_idx, eos_lprob, (const int*)ban_ids, (const int*)ban_n, (int)ban_ld));
@@ -1104,6 +1113,7 @@ extern "C" int sb_ban_step(const int32_t* seqs, int32_t seq_ld, const int32_t* s
   using namespace sb;
   SB_REQUIRE(seqs && step_ptr && table && ban_ids && ban_n && rows > 0 && seq_ld > 0 && cap > 0 && width > 0, SB_EINVAL,
              "sb_ban_step: bad args");
+  SB_CUDA_OK(prefer_shared(ban_step_kernel));
   SB_CUDA_OK(launch_k(ban_step_kernel, dim3(rows), dim3(256), 0, (cudaStream_t)stream, (const int*)seqs, (int)seq_ld,
                        (const int*)step_ptr, (const int*)table, (int)cap, (int)width, (int*)ban_ids, (int*)ban_n));
   count_launch();
@@ -1114,6 +1124,7 @@ extern "C" int sb_beam_step(const sb_beam_t* p, sb_stream_t stream) {
   using namespace sb;
   SB_REQUIRE(p && p->batch > 0 && p->beam > 0 && p->beam <= 16 && p->K > 0, SB_EINVAL, "sb_beam_step: bad args");
   SB_REQUIRE(p->step_ptr != nullptr, SB_EINVAL, "sb_beam_step: step_ptr is null");
+  SB_CUDA_OK(prefer_shared(beam_step_kernel));
   SB_CUDA_OK(launch_k(beam_step_kernel, dim3(p->batch), dim3(128), 0, (cudaStream_t)stream, *p));
   count_launch();
   return SB_OK;
@@ -1121,6 +1132,7 @@ extern "C" int sb_beam_step(const sb_beam_t* p, sb_stream_t stream) {
 
 extern "C" int sb_step_advance(int32_t* step_ptr, sb_stream_t stream) {
   SB_REQUIRE(step_ptr != nullptr, SB_EINVAL, "sb_step_advance: null");
+  SB_CUDA_OK(sb::prefer_shared(sb::step_advance_kernel));
   SB_CUDA_OK(sb::launch_k(sb::step_advance_kernel, dim3(1), dim3(1), 0, (cudaStream_t)stream, (int*)step_ptr));
   sb::count_launch();
   return SB_OK;
@@ -1129,6 +1141,7 @@ extern "C" int sb_step_advance(int32_t* step_ptr, sb_stream_t stream) {
 extern "C" int sb_store_step(const void* h, void* hist, const int32_t* step_ptr, int64_t bytes_per_step, sb_stream_t stream) {
   SB_REQUIRE(h && hist && step_ptr && bytes_per_step > 0 && bytes_per_step % 16 == 0, SB_EINVAL, "sb_store_step: bad args");
   const long long n16 = bytes_per_step / 16;
+  SB_CUDA_OK(sb::prefer_shared(sb::store_step_kernel));
   SB_CUDA_OK(sb::launch_k(sb::store_step_kernel, dim3((unsigned)((n16 + 255) / 256)), dim3(256), 0, (cudaStream_t)stream,
                           (const uint4*)h, (uint4*)hist, (const int*)step_ptr, n16));
   sb::count_launch();

@@ -219,6 +219,7 @@ extern "C" int sb_splitk_reduce_ln(const float* partials, int32_t splits, int32_
   SB_REQUIRE(partials && x && ln_w && ln_b && h && splits >= 1 && rows > 0, SB_EINVAL, "sb_splitk_reduce_ln: bad args");
   SB_REQUIRE(dim % 8 == 0 && dim <= 256 * LN_MAX_CHUNKS, SB_ENOSUP, "sb_splitk_reduce_ln: dim %d unsupported", dim);
   const int nwarp = (dim + 255) / 256;
+  SB_CUDA_OK(prefer_shared(splitk_reduce_ln_kernel));
   SB_CUDA_OK(launch_k(splitk_reduce_ln_kernel, dim3(rows), dim3(nwarp * 32), 0, (cudaStream_t)stream, partials,
                        (int)splits, (long long)rows, (long long)slice_rows, (int)dim, bias, (elem_t*)x, ln_w, ln_b, (elem_t*)h));
   count_launch();
@@ -233,6 +234,7 @@ extern "C" int sb_layernorm(const void* x, const void* res, void* y, void* sum_o
   SB_REQUIRE(dim % 8 == 0 && dim <= 256 * LN_MAX_CHUNKS, SB_ENOSUP, "sb_layernorm: dim %d unsupported (multiple of 8, <= 2048)", dim);
   const long long rows = (long long)batch * T;
   const int wpb = rows >= 4096 ? 8 : 2;  // small problems: more CTAs, shorter critical path
+  SB_CUDA_OK(prefer_shared((layernorm_kernel<SB_ACT_NONE>)));
   SB_CUDA_OK(launch_k(layernorm_kernel<SB_ACT_NONE>, dim3((unsigned)((rows + wpb - 1) / wpb)), dim3(wpb * 32), 0, (cudaStream_t)stream,
                        (const elem_t*)x, (const elem_t*)res, (elem_t*)y, (elem_t*)sum_out, w, b, (int)dim, rows, (int)T,
                        (int)in_rows, (int)in_halo, (int)out_rows, (int)out_halo, lens, (int)mask_out));

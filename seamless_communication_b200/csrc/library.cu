@@ -10,8 +10,8 @@ static thread_local char g_err[512] = "";
 long long g_launch_count = 0;
 bool pdl_enabled() {
   static int v = -1;
-  // opt-in (SB_PDL=1; not timed on H100)
-  if (v < 0) { const char* e = getenv("SB_PDL"); v = (e != nullptr && atoi(e) != 0) ? 1 : 0; }
+  // on unless SB_PDL=0 (read once per process)
+  if (v < 0) { const char* e = getenv("SB_PDL"); v = (e == nullptr || atoi(e) != 0) ? 1 : 0; }
   return v != 0;
 }
 void set_error(const char* fmt, ...) {
@@ -31,6 +31,7 @@ __global__ void cast_f32_f16_kernel(const float* __restrict__ s, elem_t* __restr
 extern "C" const char* sb_last_error(void) { return sb::g_err; }
 extern "C" int sb_version(void) { return 1; }
 extern "C" int64_t sb_launch_count(void) { return sb::g_launch_count; }
+extern "C" int sb_pdl_enabled(void) { return sb::pdl_enabled() ? 1 : 0; }
 
 extern "C" int sb_cast_f32_to_f16(const float* src, void* dst, int64_t n, sb_stream_t stream) {
   SB_REQUIRE(src && dst && n >= 0, SB_EINVAL, "sb_cast_f32_to_f16: bad args");

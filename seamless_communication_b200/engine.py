@@ -85,7 +85,11 @@ class UnitYEngine:
         self._tls = threading.local()
         self._count_lock = threading.Lock()
         self._state_lock = threading.RLock()
-        self.decode_prefetch = os.environ.get("SB_DECODE_PREFETCH", "1") != "0"
+        # L2 prefetch of the next decoder-step GEMM's weights: only without programmatic dependent launch.  With PDL the
+        # next GEMM's CTAs start under their predecessor and load their own first weight tiles, and with several lanes
+        # in flight the extra bulk prefetches only evict the other lanes' data (DESIGN section 5)
+        pdl = _lib.load().sb_pdl_enabled() != 0
+        self.decode_prefetch = os.environ.get("SB_DECODE_PREFETCH", "0" if pdl else "1") != "0"
         self.graph_kernels = 0  # kernels executed through CUDA-graph replays (bench.py: gpu_launches)
         # all six weight products of a decoder step on the transposed wgmma kernel (decode_gemm.cu) at <= 256 rows;
         # SB_DECODE_GEMM_T=0 selects the row-major wgmma chain instead
