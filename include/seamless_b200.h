@@ -201,6 +201,36 @@ int sb_nearest_centroid(const void* x, int64_t x_ld, int32_t rows, int32_t dim, 
                         sb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * UnitY2 forced aligner (models/aligner/model.py:146-277).  The embeddings are sb_vocoder_embed gathers and the convs
+ * sb_gemm calls; these two replace the distance tensor + log_softmax and the host-side alignment search.
+ * ---------------------------------------------------------------------------------------------------------------- */
+/* sb_align_lprob - out[b][j][i] = log_softmax_i(-temperature * ||f[b][j] - t[b][i]||_2) over the tokens i < text_lens[b].
+ *   f: fp32 features, frame j of row b at row b*f_rows + f_halo + j (row stride f_ld >= dim), valid for j < feat_lens[b];
+ *   t: fp32 text states in the same layout (t_rows, t_halo, t_ld), valid for i < text_lens[b].
+ *   out: fp32 [batch][T_feat][out_ld]; columns i < T_text of every frame j < T_feat are written: tokens i >= text_lens[b]
+ *   as -inf, frames j >= feat_lens[b] as 0 (every column), the rest as the log-probability.  A row with text_lens[b] <= 0
+ *   is written as 0.  Lengths above T_feat / T_text are clamped to them.
+ *   Distances are direct fp32 sums of (f - t)^2 over the channels in order (never |f|^2 + |t|^2 - 2 f.t); the softmax
+ *   statistics are fp32.  No frame or token past a row's length is read, and a row's values do not depend on the batch.
+ *   No limit on T_text or T_feat beyond int32 sizes; SB_EINVAL for batch > 65535. */
+int sb_align_lprob(const float* f, int64_t f_ld, int32_t f_rows, int32_t f_halo, const int32_t* feat_lens, const float* t,
+                   int64_t t_ld, int32_t t_rows, int32_t t_halo, const int32_t* text_lens, int32_t dim, int32_t batch,
+                   int32_t T_feat, int32_t T_text, float temperature, float* out, int64_t out_ld, sb_stream_t stream);
+/* sb_monotonic_align - _monotonic_alignment_search + bincount (model.py:212-277) per row on lp = lprob[b][:F][:N]
+ * (F = feat_lens[b], N = text_lens[b], clamped to T_feat / T_text; lprob fp32 [batch][T_feat][lp_ld]):
+ *   Q[0][j] = Q[0][j-1] + lp[j][0] (a float64 running sum), Q[i][j] = max(Q[i-1][j-1], Q[i][j-1]) + lp[j][i] in float64 for
+ *   1 <= i <= min(j, N-1), -inf elsewhere; A[F-1] = N-1, A[j] = A[j+1]-1 when Q[A[j+1]-1][j] >= Q[A[j+1]][j] (ties and
+ *   -inf == -inf to the lower index), A[j] = 0 once A[j+1] == 0.
+ *   durations: int32 [batch][T_text], durations[b][i] = #{j : A[j] = i}, 0 for i >= N.  path (optional): int32
+ *   [batch][T_feat], A[j] for j < F and -1 after.  bits: caller-sized scratch of batch * T_text * ceil(T_feat / 32) words;
+ *   bit j % 32 of word [b][i][j / 32] = (Q[i-1][j] >= Q[i][j]), written for 1 <= i <= min(j + 1, N - 1), j <= F - 2 (the
+ *   backtrack knows the comparison is true for i > j, where Q[i][j] is -inf).
+ *   A row with F <= 0 or N <= 0 gets zero durations.  One warp per row; Q takes 12 * 32 * ceil(T_text / 32) bytes of
+ *   shared memory, so SB_ENOSUP for T_text > 8192, before anything is launched. */
+int sb_monotonic_align(const float* lprob, int64_t lp_ld, int32_t batch, int32_t T_feat, int32_t T_text, const int32_t* feat_lens,
+                       const int32_t* text_lens, uint32_t* bits, int32_t* durations, int32_t* path, sb_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * sb_dwconv_ln_silu - Conformer conv module middle: causal depthwise Conv1d(k) -> LayerNorm(C) -> SiLU.
  * Replaces ConformerConvolution's depthwise_conv/layer_norm/activation (conformer_shaw/builder.py:148-156;
  * op order fairseq2.cpp:698-731 with the v2 causal + LayerNorm variant).  x,y dense (B,T,C) fp16; w [C][k] fp16.

@@ -70,6 +70,8 @@ PROTOTYPES = {
     "sb_layernorm_gelu": [c_p, c_p, c_p, c_p, i32, i32, i32, i32, i32, i32, i32, c_p, i32, c_p],
     "sb_attention_hd80": [c_p, i64, c_p, i64, c_p, i64, c_p, i64, i32, i32, i32, i32, i32, i32, i32, i32, c_p, c_p],
     "sb_nearest_centroid": [c_p, i64, i32, i32, c_p, c_p, i32, i32, c_p, c_p, c_p, c_p],
+    "sb_align_lprob": [c_p, i64, i32, i32, c_p, c_p, i64, i32, i32, c_p, i32, i32, i32, i32, f32, c_p, i64, c_p],
+    "sb_monotonic_align": [c_p, i64, i32, i32, i32, c_p, c_p, c_p, c_p, c_p, c_p],
     "sb_dwconv_ln_silu": [c_p, c_p, c_p, c_p, c_p, i32, i32, i32, i32, c_p],
     "sb_dwconv_bias_silu": [c_p, c_p, c_p, c_p, i32, i32, i32, i32, c_p],
     "sb_embed_step": [c_p, i32, c_p, c_p, c_p, f32, c_p, i32, i32, c_p],

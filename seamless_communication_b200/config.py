@@ -207,6 +207,51 @@ def small_xlsr() -> Wav2Vec2EncoderConfig:
 WAV2VEC2_ARCHS = {"xlsr2_1b_v2": xlsr2_1b_v2, "tiny_xlsr": tiny_xlsr, "small_xlsr": small_xlsr}
 
 
+# cards/nar_t2u_aligner.yaml: the unit vocabulary's languages (UnitTokenizer(num_units, unit_langs, "nar_t2u_aligner"))
+ALIGNER_UNIT_LANGS = ("arb", "ben", "cat", "ces", "cmn", "cym", "dan", "deu", "eng", "est", "fin", "fra", "hin", "ind", "ita",
+                      "jpn", "kan", "kor", "mlt", "nld", "pes", "pol", "por", "ron", "rus", "slk", "spa", "swe", "swh", "tam",
+                      "tel", "tgl", "tha", "tur", "ukr", "urd", "uzn", "vie")
+
+
+@dataclass
+class AlignerConfig:
+    """UnitY2 forced aligner (reference models/aligner/builder.py:26-87 `_aligner_nar_t2u` and cards/nar_t2u_aligner.yaml).
+    Unit vocabulary: bos 0, pad 1, eos 2, unk 3, then num_units units (u + 4), then two blocks of language symbols."""
+
+    name: str = "nar_t2u_aligner"
+    model_dim: int = 1024
+    feat_dim: int = 1024
+    num_text_layers: int = 2
+    num_feat_layers: int = 3
+    dropout: float = 0.1
+    temperature: float = 1.0
+    reduction_factor: int = 1
+    unit_vocab_size: int = 10082
+    unit_bos_idx: int = 0
+    unit_pad_idx: int = 1
+    unit_eos_idx: int = 2
+    unit_unk_idx: int = 3
+    text_vocab_size: int = 10943
+    num_units: int = 10000
+    unit_langs: Tuple[str, ...] = ALIGNER_UNIT_LANGS
+
+    def to_dict(self) -> Dict:
+        return asdict(self)
+
+
+def nar_t2u_aligner() -> AlignerConfig:
+    return AlignerConfig()
+
+
+def tiny_aligner() -> AlignerConfig:
+    """Test copy: 64 wide, the same layer counts, 256 units (vocabulary 256 + 2 * 39 + 4) and 64 characters."""
+    return AlignerConfig(name="tiny_aligner", model_dim=64, feat_dim=64, unit_vocab_size=256 + 2 * 39 + 4, text_vocab_size=64,
+                         num_units=256)
+
+
+ALIGNER_ARCHS = {"nar_t2u_aligner": nar_t2u_aligner, "tiny_aligner": tiny_aligner}
+
+
 def base_v2() -> UnitYConfig:
     return UnitYConfig()
 

@@ -84,9 +84,10 @@ def read_manifest(ctx: EvalContext) -> List[Dict[str, str]]:
     return rows
 
 
-def decode_wav(path: Path) -> Optional[torch.Tensor]:
-    """PCM WAV (8 / 16 / 32-bit integer or 32-bit float, any channel count, 16 kHz) -> (T,) fp32 in [-1, 1], channel 0.
-    None for files that cannot be decoded (the reference's pipeline yields NaN features for those and drops them)."""
+def decode_wav(path: Path, all_channels: bool = False) -> Optional[torch.Tensor]:
+    """PCM WAV (8 / 16 / 32-bit integer or 32-bit float, any channel count, 16 kHz) -> (T,) fp32 in [-1, 1], channel 0, or
+    with all_channels (C, T).  None for files that cannot be decoded (the reference's pipeline yields NaN features for
+    those and drops them)."""
     try:
         with open(path, "rb") as f:
             raw = f.read()
@@ -120,8 +121,8 @@ def decode_wav(path: Path) -> Optional[torch.Tensor]:
             x = (np.frombuffer(data, dtype=np.uint8).astype(np.float32) - 128.0) / 128.0
         else:
             return None
-        x = x[:len(x) // channels * channels].reshape(-1, channels)[:, 0]
-        return torch.from_numpy(np.ascontiguousarray(x))
+        x = x[:len(x) // channels * channels].reshape(-1, channels)
+        return torch.from_numpy(np.ascontiguousarray(x.T if all_channels else x[:, 0]))
     except (OSError, struct.error):
         return None
 

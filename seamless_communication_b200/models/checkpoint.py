@@ -209,5 +209,27 @@ def convert_wav2vec2_checkpoint(checkpoint: Mapping[str, Any]) -> Dict[str, Any]
     return {"model": out}
 
 
+def convert_unity2_aligner_checkpoint(checkpoint: Mapping[str, Any], char_pieces: Sequence[str]) -> Dict[str, Any]:
+    """UnitY2 aligner checkpoint (`unity2_aligner.pt`: text_emb_state / unit_emb_state / aligner_state) -> {"model": names of
+    UnitY2AlignmentModel} (reference models/aligner/loader.py:22-74); one that already holds
+    `model["alignment_encoder.t_conv.1.weight"]` passes through.  The character embedding rows are permuted from the
+    fairseq dictionary's sorted order to the SentencePiece order (`char_index_mapping(char_pieces)`) on a copy: the input
+    tensors are left as they are (the reference permutes them in place)."""
+    if "model" in checkpoint and "alignment_encoder.t_conv.1.weight" in checkpoint["model"]:
+        return dict(checkpoint)
+    model: Dict[str, Any] = {f"alignment_encoder.{k}": v for k, v in checkpoint["aligner_state"].items()}
+    for src, name in (("text_emb_state", "embed_text"), ("unit_emb_state", "embed_unit")):
+        for k, v in checkpoint[src].items():
+            if k != "weight":
+                raise KeyError(f"unexpected key '{k}' in {src}")
+            model[f"alignment_frontend.{name}.weight"] = v
+    idx = char_index_mapping(char_pieces)
+    ce = model["alignment_frontend.embed_text.weight"].clone()
+    with torch.inference_mode():
+        ce[torch.arange(len(idx))] = ce[idx]
+    model["alignment_frontend.embed_text.weight"] = ce
+    return {**checkpoint, "model": model}
+
+
 def load_checkpoint_file(path: str) -> Dict[str, Any]:
     return torch.load(path, map_location="cpu", weights_only=True)

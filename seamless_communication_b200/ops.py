@@ -348,6 +348,33 @@ def nearest_centroid(x: Seq, centroids: torch.Tensor, neg_half_norm: torch.Tenso
     return units
 
 
+def align_lprob(f: Seq, t: Seq, temperature: float = 1.0) -> torch.Tensor:
+    """fp32 Seqs f (frames, lens = feat_lens) and t (tokens, lens = text_lens) -> lprob (B, f.T, t.T) fp32: the log-softmax over
+    the tokens of -temperature * ||f_j - t_i||, -inf on padded tokens, 0 on padded frames (sb_align_lprob)."""
+    lib = _lib.load()
+    assert f.buf.dtype == torch.float32 and t.buf.dtype == torch.float32 and f.C == t.C and f.B == t.B
+    out = torch.empty((f.B, f.T, t.T), dtype=torch.float32, device=f.buf.device)
+    check(lib.sb_align_lprob(f.buf.data_ptr(), f.buf.stride(0), f.Tp, f.PH, f.lens.data_ptr(), t.buf.data_ptr(), t.buf.stride(0),
+                             t.Tp, t.PH, t.lens.data_ptr(), f.C, f.B, f.T, t.T, temperature, out.data_ptr(), out.stride(1),
+                             _stream()), "sb_align_lprob")
+    return out
+
+
+def monotonic_align(lprob: torch.Tensor, feat_lens: torch.Tensor, text_lens: torch.Tensor, path=False):
+    """lprob (B, T_feat, T_text) fp32, lengths int32 (B,) on the device -> durations (B, T_text) int32, and the per-frame
+    token path (B, T_feat) int32 (-1 past feat_lens) when `path` (sb_monotonic_align)."""
+    lib = _lib.load()
+    B, T_feat, T_text = lprob.shape
+    assert lprob.stride(2) == 1 and lprob.stride(0) == T_feat * lprob.stride(1)
+    dev = lprob.device
+    bits = torch.empty((B, T_text, (T_feat + 31) // 32), dtype=torch.int32, device=dev)
+    dur = torch.empty((B, T_text), dtype=torch.int32, device=dev)
+    a = torch.empty((B, T_feat), dtype=torch.int32, device=dev) if path else None
+    check(lib.sb_monotonic_align(lprob.data_ptr(), lprob.stride(1), B, T_feat, T_text, feat_lens.data_ptr(), text_lens.data_ptr(),
+                                 bits.data_ptr(), dur.data_ptr(), _p(a), _stream()), "sb_monotonic_align")
+    return (dur, a) if path else dur
+
+
 def embed_seq(ids: torch.Tensor, embed, pos, scale, dim) -> torch.Tensor:
     lib = _lib.load()
     R, L = ids.shape

@@ -23,7 +23,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 
-from .config import UnitYConfig, VocoderConfig, Wav2Vec2EncoderConfig
+from .config import AlignerConfig, UnitYConfig, VocoderConfig, Wav2Vec2EncoderConfig
 
 SPACE = "▁"
 
@@ -404,6 +404,51 @@ class _RawTextEncoder(_TextEncoder):
         return torch.tensor(ids, dtype=torch.int64, device=self.device)
 
 
+def char_pieces(text: str, is_known=None) -> List[str]:
+    """The pieces a character-level SentencePiece model (`model_type=char`, default `nmt_nfkc` normaliser) encodes `text`
+    to: NFKC; tab, newline and carriage return become spaces and other control characters are dropped; leading and
+    trailing spaces are removed and runs of spaces collapse to one; a dummy space is prepended; every space is "▁" and
+    every character is one piece, except that a run of characters the model lacks (`is_known(piece)` false) is one
+    (unknown) piece.  An empty (or all-space) text gives no pieces."""
+    import unicodedata
+    out = []
+    for ch in unicodedata.normalize("NFKC", text):
+        if ch in "\t\n\r" or unicodedata.category(ch) == "Zs":
+            out.append(" ")
+        elif unicodedata.category(ch) != "Cc":
+            out.append(ch)
+    norm = " ".join(w for w in "".join(out).split(" ") if w)
+    pieces = [SPACE] + [SPACE if ch == " " else ch for ch in norm] if norm else []
+    if is_known is None:
+        return pieces
+    out = []
+    for p in pieces:
+        if out and not is_known(p) and not is_known(out[-1]):
+            out[-1] += p
+        else:
+            out.append(p)
+    return out
+
+
+class RawCharEncoder:
+    """The character model's raw encoder (fairseq2 SentencePieceEncoder without prefix or suffix): one id per piece of
+    `char_pieces`, the unk id for a run of characters the model lacks.  `encode_as_tokens` gives the pieces themselves.
+    model: anything with `token_to_index(piece)` that returns `unk_idx` for a piece it does not hold."""
+
+    def __init__(self, model, unk_idx: int, device=None):
+        self.model, self.unk_idx, self.device = model, unk_idx, device
+
+    def _known(self, piece: str) -> bool:
+        return self.model.token_to_index(piece) != self.unk_idx
+
+    def __call__(self, text: str) -> torch.Tensor:
+        return torch.tensor([self.model.token_to_index(p) for p in char_pieces(text, self._known)], dtype=torch.int64,
+                            device=self.device)
+
+    def encode_as_tokens(self, text: str) -> List[str]:
+        return char_pieces(text, self._known)
+
+
 class SyntheticCharTokenizer:
     """Char-level piece model (reference: models/unity/char_tokenizer.py:30; vocab 10943 for v2)."""
 
@@ -414,6 +459,7 @@ class SyntheticCharTokenizer:
         assert len(pieces) == vocab_size, (len(pieces), vocab_size)
         self.model = _PieceModel(pieces, 0)
         self.vocab_info = VocabularyInfo(size=vocab_size, unk_idx=0, bos_idx=2, eos_idx=3, pad_idx=1)
+
 
 
 def make_tokenizers(cfg: UnitYConfig) -> Tuple[SyntheticNllbTokenizer, SyntheticCharTokenizer]:
@@ -495,3 +541,22 @@ def make_kmeans_centroids(num: int, dim: int, seed: int = 4, scale: float = 1.0)
     """(num, dim) fp32 centroids on the fp16 grid (the layout KmeansModel's `.npy` is transposed to, kmeans.py:17-19)."""
     g = torch.Generator().manual_seed(seed)
     return _round_fp16(torch.randn(num, dim, generator=g) * scale)
+
+
+def make_aligner_state_dict(cfg: AlignerConfig, seed: int = 5, embed_std: float = 1.0) -> Dict[str, torch.Tensor]:
+    """Random-init UnitY2 aligner parameters under the reference's names (models/aligner/model.py:25-144 module tree:
+    alignment_frontend.embed_{text,unit}, alignment_encoder.{t,f}_conv.<Sequential index>) on the fp16 grid."""
+    I = _Init(seed)
+    M = cfg.model_dim
+    I.normal("alignment_frontend.embed_text.weight", (cfg.text_vocab_size, M), embed_std)
+    I.normal("alignment_frontend.embed_unit.weight", (cfg.unit_vocab_size, cfg.feat_dim), embed_std)
+    # Sequential indices: Permute12, then (Conv1d, ReLU, Dropout) per k3 layer, then Conv1d(k1), Dropout, Permute12
+    for i in range(cfg.num_text_layers):
+        k = 3 if i < cfg.num_text_layers - 1 else 1
+        I.conv(f"alignment_encoder.t_conv.{1 + 3 * i}", M, M, k)
+    c_in = cfg.feat_dim
+    for i in range(cfg.num_feat_layers):
+        k = 3 if i < cfg.num_feat_layers - 1 else 1
+        I.conv(f"alignment_encoder.f_conv.{1 + 3 * i}", M, c_in, k)
+        c_in = M
+    return I.sd
