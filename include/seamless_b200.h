@@ -272,6 +272,15 @@ int sb_decode_self_attn(const void* qkv, const float* qkv_partials, int32_t spli
 int sb_decode_cross_attn(const void* q, const float* q_partials, int32_t splits, int64_t slice_rows, const float* q_bias,
                          const void* k, const void* v, int64_t kv_ld, const int32_t* enc_lens, int32_t s_enc, void* out,
                          int32_t rows, int32_t beam, int32_t heads, sb_stream_t stream);
+/* head-summed attention weights of the same cross-attention, for token timestamps: with q gathered from q_partials +
+ * q_bias as sb_decode_cross_attn gathers it (fp16 after the fp32 sum), writes the fp32 slab hist[*step_ptr] of hist
+ * [max_len][rows][s_enc]:  hist[*step_ptr][r][t] = sum over heads h (ascending) of softmax_t(q_h . k_h[t] / 8) for
+ * t < len = min(enc_lens[r / beam], s_enc) (s_enc without enc_lens), and 0 for len <= t < s_enc.  Deterministic (no
+ * atomics).  Keys at t >= len are never read.  k 16-byte aligned, kv_ld a multiple of 8.  SB_ENOSUP past 48 KB of
+ * shared memory: heads * 128 + s_enc * 8 bytes (s_enc <= 5888 at 16 heads). */
+int sb_decode_cross_attn_weights(const float* q_partials, int32_t splits, int64_t slice_rows, const float* q_bias, const void* k,
+                                 int64_t kv_ld, const int32_t* enc_lens, int32_t s_enc, const int32_t* step_ptr, float* hist,
+                                 int32_t rows, int32_t beam, int32_t heads, sb_stream_t stream);
 /* per row: log-softmax statistics and the top-K candidates of an fp32 logit row.
  *   cand_val [rows][K] = lprob, cand_idx [rows][K]; eos_lprob[rows] = lprob of eos; pad is never a candidate. */
 int sb_logits_topk(const float* logits, int64_t ld, int32_t rows, int32_t vocab, int32_t pad_idx, int32_t eos_idx,
@@ -325,8 +334,30 @@ typedef struct {
   const int32_t* len_budget; /* [1] on the device or NULL: the search's length budget (<= max_len; EOS forced at step
                                 budget-2, no step past budget-1), so one captured step serves every budget up to the
                                 allocated max_len, which stays the row stride of the arrays above.  NULL: max_len */
+  float* fin_scores;   /* [B][beam][max_len] or NULL: per finished hypothesis, its cumulative scores scores[row][0 .. step]
+                          and, at step + 1, the unnormalised score of its EOS */
 } sb_beam_t;
 int sb_beam_step(const sb_beam_t* p, sb_stream_t stream);
+
+/* Token start bins of the transcriber (inference/transcriber.py:178-235) for each row's winning hypothesis; one CTA per
+ * row.  Row b has n = n_tok[b] generated tokens (its EOS excluded), F = min(enc_lens[b], s_enc) - 2 encoder frames
+ * (s_enc - 2 without enc_lens) and W[t] = hist[t][slots[b][t]] (hist fp32 [max_len][rows][s_enc], as written by
+ * sb_decode_cross_attn_weights; slots int32 [batch][slots_ld], the winner's cache slot of every position).  It builds
+ * A[k][j] = W[P-1+k][1+j] in float64 (P = prefix_len, k < n, j < F), divides each column by its sum over k = 0 .. n-1
+ * taken in that order (a zero column stays 0), applies a width x width median filter with zero padding, takes the
+ * smallest k attaining each column's maximum, runs generate_lis over the pairs (c[j], -j), and writes
+ * starts[b][k] (int32 [batch][starts_ld]): the bin j of the path's pair with c[j] == k, else the previous token's start
+ * (token 0: 0).  The result equals a float64 restatement bit for bit.
+ * Only hist[P-1 .. P+n-2][slot][1 .. F] is read.  scratch holds batch x scratch_ld doubles.  Rows with n = 0 or F < 1
+ * write nothing, nor do rows with n > starts_ld, P - 1 + n > slots_ld or n * F > scratch_ld.
+ * Limits (SB_ENOSUP before launching): width odd and at most SB_TS_MAX_WIDTH (SB_EINVAL for an even width or one below
+ * 1), s_enc - 2 <= SB_TS_MAX_FRAMES (12 bytes of shared memory per frame).  n is bounded only by the buffers: a
+ * 1024-position search fits, and a 20 s input has s_enc = 125 encoder frames (F = 123). */
+#define SB_TS_MAX_WIDTH 7
+#define SB_TS_MAX_FRAMES 4096
+int sb_token_timestamps(const float* hist, int32_t rows, int32_t s_enc, const int32_t* slots, int32_t slots_ld,
+                        const int32_t* n_tok, const int32_t* enc_lens, int32_t prefix_len, int32_t batch, int32_t width,
+                        double* scratch, int64_t scratch_ld, int32_t* starts, int32_t starts_ld, sb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * NAR T2U frontend (models/unity/nar_decoder_frontend.py:130-334, length_regulator.py:24-39,275-321) on device.

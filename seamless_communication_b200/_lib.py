@@ -44,7 +44,7 @@ class BeamDesc(C.Structure):
         ("cand_val", c_p), ("cand_idx", c_p), ("eos_lprob", c_p),
         ("seqs", c_p), ("scores", c_p), ("anc", c_p),
         ("fin_count", c_p), ("fin_score", c_p), ("fin_len", c_p), ("fin_seqs", c_p), ("active", c_p),
-        ("fin_anc", c_p), ("n_active", c_p), ("len_budget", c_p),
+        ("fin_anc", c_p), ("n_active", c_p), ("len_budget", c_p), ("fin_scores", c_p),
     ]
 
 
@@ -80,9 +80,11 @@ PROTOTYPES = {
     "sb_embed_seq": [c_p, i32, i32, c_p, c_p, f32, c_p, i32, i32, c_p],
     "sb_decode_self_attn": [c_p, c_p, i32, i64, c_p, c_p, c_p, c_p, i32, c_p, i32, c_p, i32, i32, c_p],
     "sb_decode_cross_attn": [c_p, c_p, i32, i64, c_p, c_p, c_p, i64, c_p, i32, c_p, i32, i32, i32, c_p],
+    "sb_decode_cross_attn_weights": [c_p, i32, i64, c_p, c_p, i64, c_p, i32, c_p, c_p, i32, i32, i32, c_p],
     "sb_logits_topk": [c_p, i64, i32, i32, i32, i32, i32, f32, i32, c_p, c_p, c_p, c_p],
     "sb_logits_topk_tiles": [c_p, i64, c_p, i32, i32, i32, i32, i32, f32, i32, c_p, c_p, c_p, c_p],
     "sb_beam_step": [C.POINTER(BeamDesc), c_p],
+    "sb_token_timestamps": [c_p, i32, i32, c_p, i32, c_p, c_p, i32, i32, i32, c_p, i64, c_p, i32, c_p],
     "sb_ban_step": [c_p, i32, c_p, i32, c_p, i32, i32, c_p, c_p, c_p],
     "sb_logits_topk_ban": [c_p, i64, i32, i32, i32, i32, i32, f32, i32, c_p, c_p, c_p, c_p, c_p, i32, c_p],
     "sb_logits_topk_tiles_ban": [c_p, i64, c_p, i32, i32, i32, i32, i32, f32, i32, c_p, c_p, c_p, c_p, c_p, i32, c_p],

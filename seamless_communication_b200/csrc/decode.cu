@@ -852,6 +852,11 @@ __global__ void __launch_bounds__(128) beam_step_kernel(const sb_beam_t p) {
             for (int t = 0; t < step; ++t) fa[t] = p.anc[(long long)row * ML + t];
             fa[step] = row;
           }
+          if (p.fin_scores != nullptr) {  // cumulative (unnormalised) scores of this hypothesis, its EOS at step + 1
+            float* fs = p.fin_scores + ((long long)b * beam + fin) * ML;
+            for (int t = 0; t <= step; ++t) fs[t] = p.scores[(long long)row * ML + t];
+            fs[step + 1] = best;
+          }
           p.fin_len[b * beam + fin] = step + 2;
           p.fin_score[b * beam + fin] = best / powf((float)(step + 1), p.len_penalty);
           ++fin;
@@ -934,6 +939,81 @@ __global__ void store_step_kernel(const uint4* __restrict__ h, uint4* __restrict
 __global__ void step_advance_kernel(int* step_ptr) {
   pdl_sync();
   *step_ptr += 1;
+}
+
+// Head-summed cross-attention weights of one decoder step, kept for the transcriber's token timestamps (the reference hooks
+// the last decoder layer's encoder-decoder attention, inference/transcriber.py:39-57):
+//   hist[*step_ptr][r][t] = sum_h softmax_h(q_h . k_h[t] / 8)[t]  for t < len(r / beam), 0 for len <= t < s_enc.
+// One CTA per row.  Every key belongs to one thread in every pass, heads are added in ascending order and the block
+// reductions combine the warps in a fixed order, so the result is the same bits on every run (no atomics).  q is gathered
+// from the split-K partials as the cross-attention kernels gather it (fp32 sum + bias, rounded to fp16).
+constexpr int XW_THREADS = 256;
+
+template <bool MAX>
+__device__ __forceinline__ float xw_block_reduce(float v, float* s_red) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  v = MAX ? warp_max(v) : warp_sum(v);
+  if (lane == 0) s_red[warp] = v;
+  __syncthreads();
+  float r = s_red[0];
+  for (int i = 1; i < XW_THREADS / 32; ++i) r = MAX ? fmaxf(r, s_red[i]) : r + s_red[i];
+  __syncthreads();  // s_red is rewritten by the next reduction
+  return r;
+}
+
+__global__ void __launch_bounds__(XW_THREADS) decode_cross_attn_weights_kernel(const float* __restrict__ part, int splits,
+                                                                               long long slice_rows, const float* __restrict__ bias,
+                                                                               const elem_t* __restrict__ k, long long kv_ld,
+                                                                               const int* __restrict__ enc_lens, int s_enc,
+                                                                               const int* __restrict__ step_ptr,
+                                                                               float* __restrict__ hist, int rows, int beam, int heads) {
+  extern __shared__ __align__(16) unsigned char xw_smem[];  // q [heads][64] fp16, then scores [s_enc], head sum [s_enc]
+  __shared__ float s_red[XW_THREADS / 32];
+  pdl_sync();
+  const int r = blockIdx.x, b = r / beam;
+  const int warp = threadIdx.x >> 5;
+  const int dim = heads * HD;
+  elem_t* qs = reinterpret_cast<elem_t*>(xw_smem);
+  float* sc = reinterpret_cast<float*>(qs + (size_t)heads * HD);
+  float* acc = sc + s_enc;
+  const int len = enc_lens ? min(enc_lens[b], s_enc) : s_enc;
+  for (int h = warp; h < heads; h += XW_THREADS / 32) gather_head_vec(part, splits, slice_rows, dim, bias, r, h * HD, qs + h * HD);
+  for (int t = threadIdx.x; t < len; t += XW_THREADS) acc[t] = 0.f;
+  __syncthreads();
+  const elem_t* kb = k + (long long)b * s_enc * kv_ld;
+  for (int h = 0; h < heads; ++h) {
+    const uint4* qh = reinterpret_cast<const uint4*>(qs + h * HD);
+    float mx = -INFINITY;
+    for (int t = threadIdx.x; t < len; t += XW_THREADS) {
+      const uint4* kp = reinterpret_cast<const uint4*>(kb + (long long)t * kv_ld + h * HD);
+      float a = 0.f;
+#pragma unroll
+      for (int c = 0; c < HD / 8; ++c) {
+        const uint4 ku = kp[c], qu = qh[c];
+        const __half2* kh = reinterpret_cast<const __half2*>(&ku);
+        const __half2* qq = reinterpret_cast<const __half2*>(&qu);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float2 kf = __half22float2(kh[e]), qf = __half22float2(qq[e]);
+          a += qf.x * kf.x + qf.y * kf.y;
+        }
+      }
+      a *= 0.125f;
+      sc[t] = a;
+      mx = fmaxf(mx, a);
+    }
+    mx = xw_block_reduce<true>(mx, s_red);
+    float sum = 0.f;
+    for (int t = threadIdx.x; t < len; t += XW_THREADS) {
+      const float e = expf(sc[t] - mx);
+      sc[t] = e;
+      sum += e;
+    }
+    const float inv = 1.f / xw_block_reduce<false>(sum, s_red);
+    for (int t = threadIdx.x; t < len; t += XW_THREADS) acc[t] += sc[t] * inv;
+  }
+  float* dst = hist + ((long long)(*step_ptr) * rows + r) * s_enc;
+  for (int t = threadIdx.x; t < s_enc; t += XW_THREADS) dst[t] = t < len ? acc[t] : 0.f;
 }
 
 }  // namespace sb
@@ -1032,6 +1112,24 @@ extern "C" int sb_decode_cross_attn(const void* q, const float* q_partials, int3
                        (const elem_t*)q, q_partials, (int)splits, (long long)slice_rows, q_bias, (const elem_t*)k,
                        (const elem_t*)v, (long long)kv_ld, (const int*)enc_lens, (int)s_enc,
                        (elem_t*)out, (int)rows, (int)beam, (int)heads));
+  count_launch();
+  return SB_OK;
+}
+
+extern "C" int sb_decode_cross_attn_weights(const float* q_partials, int32_t splits, int64_t slice_rows, const float* q_bias,
+                                            const void* k, int64_t kv_ld, const int32_t* enc_lens, int32_t s_enc,
+                                            const int32_t* step_ptr, float* hist, int32_t rows, int32_t beam, int32_t heads,
+                                            sb_stream_t stream) {
+  using namespace sb;
+  SB_REQUIRE(q_partials && q_bias && splits >= 1 && k && step_ptr && hist && rows > 0 && beam > 0 && rows % beam == 0 &&
+                 heads > 0 && s_enc > 0 && kv_ld % 8 == 0 && ((uintptr_t)k % 16) == 0,
+             SB_EINVAL, "sb_decode_cross_attn_weights: bad args");
+  const size_t smem = (size_t)heads * HD * sizeof(elem_t) + (size_t)2 * s_enc * sizeof(float);
+  SB_REQUIRE(smem <= 48 * 1024, SB_ENOSUP, "sb_decode_cross_attn_weights: s_enc %d with %d heads too large", s_enc, heads);
+  SB_CUDA_OK(prefer_shared(decode_cross_attn_weights_kernel));
+  SB_CUDA_OK(launch_k(decode_cross_attn_weights_kernel, dim3(rows), dim3(XW_THREADS), smem, (cudaStream_t)stream, q_partials,
+                       (int)splits, (long long)slice_rows, q_bias, (const elem_t*)k, (long long)kv_ld, (const int*)enc_lens,
+                       (int)s_enc, (const int*)step_ptr, hist, (int)rows, (int)beam, (int)heads));
   count_launch();
   return SB_OK;
 }

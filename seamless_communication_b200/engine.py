@@ -328,10 +328,11 @@ class UnitYEngine:
         return [self._lin(enc, f"text_decoder.layers.{i}.encoder_decoder_attn.kv", 2 * self.M)
                 for i in range(self.cfg.dec_layers)]
 
-    def _decoder_step_forward(self, st):
+    def _decoder_step_forward(self, st, record=False):
         """One incremental decoder step for R rows; all shapes static, step index read from st['step'] on device.
         The three residual GEMMs of a layer (self-attn out, cross-attn out, FFN out) run split-K so that all SMs stream
-        weights even at M = R rows, and their reduction (+bias, +residual) is fused into the LayerNorm that follows."""
+        weights even at M = R rows, and their reduction (+bias, +residual) is fused into the LayerNorm that follows.
+        `record`: the last layer's head-summed cross-attention weights go to st["attn_hist"][step] (token timestamps)."""
         lib = _lib.load()
         c, M, H = self.cfg, self.M, self.H
         R, stream = st["R"], ops._stream()
@@ -365,6 +366,9 @@ class UnitYEngine:
                                            kv.data_ptr(), kv[:, M:].data_ptr(), kv.stride(0), ops._p(st["enc_lens"]),
                                            st["S_enc"], st["att"].buf.data_ptr(), R, st["beam"], H, stream),
                   "sb_decode_cross_attn")
+            if record and last:  # reads the q partials before the next product overwrites them
+                ops.decode_cross_attn_weights(part, S_ATT, SR, w[p + ".encoder_decoder_attn.q_proj.b"], kv, st["enc_lens"],
+                                              st["S_enc"], st["step"], st["attn_hist"], R, st["beam"], H)
             ops.gemm_splitk(st["att"], w[p + ".encoder_decoder_attn.output_proj.w"], M, S_ATT, part,
                             prefetch=w[p + ".ffn.inner_proj.w"] if pf else None, transposed=st["gemm_t"])
             ops.splitk_reduce_ln(part, S_ATT, w[p + ".encoder_decoder_attn.output_proj.b"], x, w[p + ".ffn_layer_norm.w"],
@@ -453,7 +457,7 @@ class UnitYEngine:
         # the top-K kernel returns at most 16 candidates per row and the step needs 2*beam + 1 (one spare for a blocked EOS)
         if 2 * beam + 1 > 16:
             raise ValueError(f"beam_size {beam} is not supported by the top-K kernel (at most 7)")
-        st = dict(R=R, ML=ML, beam=beam, K=K, S_enc=S_enc, B=B, P=P, unk_penalty=0.0)
+        st = dict(R=R, ML=ML, beam=beam, K=K, S_enc=S_enc, B=B, P=P, unk_penalty=0.0, key=key)
         st["enc_lens"] = torch.zeros(B, dtype=I32, device=dev) if has_lens else None
         st["cross_kv"] = [Seq(B, S_enc, 2 * M) for _ in range(c.dec_layers)]
         st["seqs"] = torch.zeros((R, ML), dtype=I32, device=dev)
@@ -486,6 +490,7 @@ class UnitYEngine:
                    len=torch.zeros((B, beam), dtype=I32, device=dev), seqs=torch.zeros((B, beam, ML), dtype=I32, device=dev),
                    active=torch.ones(B, dtype=I32, device=dev), n_active=torch.zeros((1,), dtype=I32, device=dev))
         fin["anc"] = torch.zeros((B, beam, ML), dtype=I32, device=dev)
+        fin["scores"] = torch.zeros((B, beam, ML), dtype=torch.float32, device=dev)  # cumulative scores of each finished hypothesis
         st["hist"] = torch.empty((ML, R, M), dtype=F16, device=dev)  # final-LN decoder state of every step
         st["fin"] = fin
         d = BeamDesc()
@@ -496,9 +501,11 @@ class UnitYEngine:
         d.fin_count, d.fin_score, d.fin_len = fin["count"].data_ptr(), fin["score"].data_ptr(), fin["len"].data_ptr()
         d.fin_seqs, d.active, d.n_active = fin["seqs"].data_ptr(), fin["active"].data_ptr(), fin["n_active"].data_ptr()
         d.fin_anc, d.len_budget = fin["anc"].data_ptr(), st["budget"].data_ptr()
+        d.fin_scores = fin["scores"].data_ptr()
         st["beam_desc"] = d
-        st["g_fwd"] = st["g_sel"] = st["g_sel_ban"] = None
-        st["n_fwd"] = st["n_sel"] = st["n_sel_ban"] = 0
+        st["g_fwd"] = st["g_sel"] = st["g_sel_ban"] = st["g_fwd_attn"] = None
+        st["n_fwd"] = st["n_sel"] = st["n_sel_ban"] = st["n_fwd_attn"] = 0
+        st["attn_hist"], st["attn_on"] = None, False  # [ML][R][S_enc] fp32, allocated by the first recording search
         st["ban"], st["ban_on"] = None, False
         self._graphs[key] = st
         self._evict_search_states(keep=key)
@@ -579,6 +586,21 @@ class UnitYEngine:
                 self._decoder_step_select(st, ban=True)
             st["n_sel_ban"] = ops.launch_count() - n0
 
+    def _capture_attn(self, st):
+        """Capture the forward half with the cross-attention weights recorded (sb_decode_cross_attn_weights after the last
+        layer's cross-attention); searches that do not record keep replaying g_fwd."""
+        with _CAPTURE_LOCK:
+            s = torch.cuda.Stream()
+            s.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(s):
+                self._decoder_step_forward(st, record=True)
+            torch.cuda.current_stream().wait_stream(s)
+            n0 = ops.launch_count()
+            st["g_fwd_attn"] = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(st["g_fwd_attn"], capture_error_mode="thread_local"):
+                self._decoder_step_forward(st, record=True)
+            st["n_fwd_attn"] = ops.launch_count() - n0
+
     def _set_bans(self, st, banned):
         """Pack the banned sequences into the state's device table ([count][lengths x cap][cap rows of `width` tokens,
         right-aligned]) with one asynchronous host-to-device copy.  The buffers, and the graph captured on them, are
@@ -614,7 +636,7 @@ class UnitYEngine:
         st["step"].zero_()
 
     def _search_prepare(self, st, enc: Seq, enc_lens, prefix, len_penalty, unk_penalty, min_seq_len, use_graph, max_len,
-                        banned=None):
+                        banned=None, record=False):
         """(Re)initialise one cached search state in place for the sentences of `enc` and a length budget `max_len`
         (<= the state's allocated length); capture its graphs if needed."""
         c, M = self.cfg, self.M
@@ -627,6 +649,11 @@ class UnitYEngine:
             st["g_fwd"] = st["g_sel"] = st["g_sel_ban"] = None  # scalar options are baked into the captured select graphs
             st["unk_cap"] = float(unk_penalty)
         st["ban_on"] = bool(banned)
+        st["attn_on"] = record
+        if record and st["attn_hist"] is None:
+            st["attn_hist"] = torch.zeros((st["ML"], st["R"], st["S_enc"]), dtype=torch.float32, device=self.device)
+            with self._state_lock:  # the cache budget now counts the history too
+                self._evict_search_states(keep=st["key"])
         if banned:
             self._set_bans(st, banned)
         if enc_lens is not None:
@@ -640,17 +667,21 @@ class UnitYEngine:
         if use_graph and banned and st["g_sel_ban"] is None:
             self._capture_ban(st)
             self._search_reset(st, prefix)
+        if use_graph and record and st["g_fwd_attn"] is None:
+            self._capture_attn(st)
+            self._search_reset(st, prefix)
 
     def _search_step(self, st, use_graph, select=True):
-        ban = st["ban_on"]
+        ban, rec = st["ban_on"], st["attn_on"]
         if use_graph:
-            st["g_fwd"].replay()
+            st["g_fwd_attn" if rec else "g_fwd"].replay()
             if select:
                 st["g_sel_ban" if ban else "g_sel"].replay()
             with self._count_lock:
-                self.graph_kernels += st["n_fwd"] + ((st["n_sel_ban"] if ban else st["n_sel"]) if select else 0)
+                self.graph_kernels += (st["n_fwd_attn"] if rec else st["n_fwd"]) + \
+                    ((st["n_sel_ban"] if ban else st["n_sel"]) if select else 0)
         else:
-            self._decoder_step_forward(st)
+            self._decoder_step_forward(st, record=rec)
             if select:
                 self._decoder_step_select(st, ban=ban)
 
@@ -681,7 +712,7 @@ class UnitYEngine:
     @torch.inference_mode()
     def beam_search(self, enc: Seq, enc_lens, prefix: List[int], beam=5, soft_max=(1, 200), hard_max=1024,
                     len_penalty=1.0, unk_penalty=0.0, min_seq_len=1, use_graph=True, cross_kv=None, state_len=None,
-                    banned=None):
+                    banned=None, record_attention=False):
         """Device-resident beam search.  Returns per sentence the finished hypotheses [(score, ids)], best first
         (semantics: fairseq2.cpp:1371-1608; see decode.cu).  `cross_kv` is ignored (kept for API stability): the
         static cross-attention K/V of the cached search state are recomputed from `enc`.
@@ -689,7 +720,9 @@ class UnitYEngine:
         min(hard_max, a*S_enc + b); the budget is then a device scalar of the state, so searches whose budgets differ
         share one state and its captured graphs.  None: the state is sized by the budget.
         `banned`: token-id sequences of fairseq2's BannedSequenceProcessor, applied at every selecting step (not in the
-        prefix bootstrap): a row whose last n-1 tokens equal a sequence's first n-1 cannot take its last token."""
+        prefix bootstrap): a row whose last n-1 tokens equal a sequence's first n-1 cannot take its last token.
+        `record_attention`: every step also keeps the last decoder layer's head-summed cross-attention weights, for
+        `token_timestamps` (one more kernel per step, on a third captured graph of the state)."""
         if banned is not None:
             banned = [[int(t) for t in (x.tolist() if isinstance(x, torch.Tensor) else x)] for x in banned]
             V = self.cfg.text_vocab
@@ -709,7 +742,8 @@ class UnitYEngine:
         assert enc.PH == 0 and enc.Tp == enc.T, "encoder output must be a halo-free Seq"
         ML_state = ML if state_len is None else max(ML, int(state_len))
         st = self._search_state(B, S_enc, ML_state, beam, P, enc_lens is not None, use_graph)
-        self._search_prepare(st, enc, enc_lens, prefix, len_penalty, unk_penalty, min_seq_len, use_graph, ML, banned)
+        self._search_prepare(st, enc, enc_lens, prefix, len_penalty, unk_penalty, min_seq_len, use_graph, ML, banned,
+                             bool(record_attention))
         n_steps = ML - 1 - (P - 1)
         for i in range(P - 1):
             self._search_bootstrap_step(st, prefix, i, use_graph)
@@ -745,6 +779,54 @@ class UnitYEngine:
         lens = torch.tensor(lengths, dtype=I32, device=dev)
         out = out * (t_idx < lens[:, None].to(torch.int64))[:, :, None].to(out.dtype)             # zero the padding rows
         return Seq(B, L, M, lens=lens, buf=out.reshape(B * L, M).contiguous())
+
+    def _best_hypotheses(self, st):
+        """(index into the batch, winner index >= 0, generated-token count n excluding the EOS) of the last search."""
+        best = st["best_fin"]
+        sel = torch.tensor([max(j, 0) for j in best], dtype=torch.int64, device=self.device)
+        lens = st["fin"]["len"][torch.arange(st["B"], device=self.device), sel].tolist()
+        n = [ln - st["P"] - 1 if j >= 0 else 0 for ln, j in zip(lens, best)]
+        return sel, n
+
+    def _recorded_state(self):
+        st = self._last_search_state
+        if st is None or not st["attn_on"]:
+            raise RuntimeError("the last beam_search of this thread did not run with record_attention=True")
+        return st
+
+    @torch.inference_mode()
+    def harvest_attention(self) -> Tuple[torch.Tensor, List[int]]:
+        """The recorded cross-attention rows of each sentence's best hypothesis: (B, max n, S_enc) fp32 on the device, row k
+        of sentence b being decoder position P-1+k (the step that chose generated token k), zeros past n; and the
+        generated-token counts n (EOS excluded).  Gathered along the winner's cache slots (fin_anc)."""
+        st = self._recorded_state()
+        sel, n = self._best_hypotheses(st)
+        B, P, dev = st["B"], st["P"], self.device
+        L = max(max(n), 1)
+        slots = st["fin"]["anc"][torch.arange(B, device=dev), sel][:, P - 1:P - 1 + L].to(torch.int64)
+        pos = torch.arange(P - 1, P - 1 + L, device=dev)[None, :].expand(B, L)
+        out = st["attn_hist"][pos, slots]
+        keep = torch.arange(L, device=dev)[None, :] < torch.tensor(n, device=dev)[:, None]
+        return out * keep[:, :, None].to(out.dtype), n
+
+    @torch.inference_mode()
+    def token_timestamps(self, filter_width: int = 3) -> List[Tuple[List[int], List[float]]]:
+        """Per sentence of the last (recording) beam search: the start bin of every generated token of its best hypothesis
+        (sb_token_timestamps: inference/transcriber.py's _extract_timestamps on the device, over F = len - 2 encoder
+        frames) and its per-token scores float32(cum[P+k] - cum[P+k-1]) of the hypothesis' cumulative scores."""
+        st = self._recorded_state()
+        sel, n = self._best_hypotheses(st)
+        B, P, dev = st["B"], st["P"], self.device
+        ar = torch.arange(B, device=dev)
+        slots = st["fin"]["anc"][ar, sel].contiguous()
+        starts = ops.token_timestamps(st["attn_hist"], slots, torch.tensor(n, dtype=I32, device=dev), st["enc_lens"], P,
+                                      filter_width).cpu()
+        cum = st["fin"]["scores"][ar, sel].cpu()
+        out = []
+        for b in range(B):
+            c = cum[b, P - 1:P + n[b]]
+            out.append((starts[b, :n[b]].tolist(), (c[1:] - c[:-1]).tolist()))
+        return out
 
     # ------------------------------------------------------------------------------------------ a10 teacher-forced pass
     @torch.inference_mode()

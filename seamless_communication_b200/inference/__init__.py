@@ -1,2 +1,3 @@
 from .generator import BannedSequenceProcessor, SequenceGeneratorOptions, UnitYGenerator
 from .translator import BatchedSpeechOutput, Modality, Task, Translator
+from .transcriber import Transcriber, Transcription, TranscriptionToken, TranscriptionTokenStats

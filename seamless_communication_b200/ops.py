@@ -375,6 +375,37 @@ def monotonic_align(lprob: torch.Tensor, feat_lens: torch.Tensor, text_lens: tor
     return (dur, a) if path else dur
 
 
+def decode_cross_attn_weights(q_partials: torch.Tensor, splits: int, slice_rows: int, q_bias: torch.Tensor, k: torch.Tensor,
+                              enc_lens: Optional[torch.Tensor], s_enc: int, step: torch.Tensor, hist: torch.Tensor, rows: int,
+                              beam: int, heads: int) -> None:
+    """hist[step][r] = the head-summed softmax weights of row r's cross-attention over its utterance's s_enc frames
+    (sb_decode_cross_attn_weights).  k: the K half of the cross K|V buffer ((B * s_enc, >= heads * 64) view)."""
+    check(_lib.load().sb_decode_cross_attn_weights(q_partials.data_ptr(), splits, slice_rows, q_bias.data_ptr(), k.data_ptr(),
+                                                   k.stride(0), _p(enc_lens), s_enc, step.data_ptr(), hist.data_ptr(), rows, beam,
+                                                   heads, _stream()), "sb_decode_cross_attn_weights")
+
+
+def token_timestamps(hist: torch.Tensor, slots: torch.Tensor, n_tok: torch.Tensor, enc_lens: Optional[torch.Tensor],
+                     prefix_len: int, width: int) -> torch.Tensor:
+    """Start bins (B, max(n_tok)) int32 of each row's tokens from the attention history hist (max_len, rows, s_enc) fp32
+    along the slot table slots (B, >= prefix_len - 1 + max(n_tok)) int32 (sb_token_timestamps).  Entries past a row's n_tok,
+    and every entry of a row with fewer than three encoder frames, are 0."""
+    lib = _lib.load()
+    _, rows, s_enc = hist.shape
+    B = slots.shape[0]
+    dev = hist.device
+    n_host = n_tok.tolist()
+    n_max = max(max(n_host), 1)
+    lens = [min(int(x), s_enc) for x in enc_lens.tolist()] if enc_lens is not None else [s_enc] * B
+    per_row = max([max(n, 0) * max(f - 2, 0) for n, f in zip(n_host, lens)] + [1])
+    scratch = torch.empty((B, per_row), dtype=torch.float64, device=dev)
+    starts = torch.zeros((B, n_max), dtype=torch.int32, device=dev)
+    check(lib.sb_token_timestamps(hist.data_ptr(), rows, s_enc, slots.data_ptr(), slots.stride(0), n_tok.data_ptr(), _p(enc_lens),
+                                  prefix_len, B, width, scratch.data_ptr(), per_row, starts.data_ptr(), n_max, _stream()),
+          "sb_token_timestamps")
+    return starts
+
+
 def embed_seq(ids: torch.Tensor, embed, pos, scale, dim) -> torch.Tensor:
     lib = _lib.load()
     R, L = ids.shape
