@@ -432,6 +432,30 @@ int sb_avgpool_time(const void* x, void* y, int32_t batch, int32_t T, int32_t C,
 int sb_pchoose(const void* q_energy, const void* k_energy, float* p, int32_t S, int32_t Sp, int32_t heads,
                float energy_bias, float temperature, sb_stream_t stream);
 
+/* Many streams at once (one policy round of a multi-stream server).
+ *   sb_pchoose_ragged: p[b][h] = sb_pchoose's value of stream b's newest target position q_lens[b] - 1 against its last pooled
+ *     source position k_lens[b] - 1, the one entry the policy's decision reads.  q (batch * q_rows, H*64) and k
+ *     (batch * k_rows, H*64) in sequence layout; q_lens / k_lens int32 [batch] on the device, in [1, q_rows] / [1, k_rows]
+ *     (a length outside that range gives NaN); no row past a stream's lengths is read.  Bit-identical to sb_pchoose.
+ *   sb_policy_decide: one CTA per stream b writes out[b] = {token, decision value as float bits} (int32 [batch][2]).
+ *     ctl[b] (int32 [batch][SB_POLICY_CTL]) = {4 blocked ids (-1 = unused), method, layer0}.
+ *     token = argmax of logits[b][0..vocab) (fp32, row stride ld) with the blocked ids at -inf, NaN first and ties to the
+ *     lowest index as in torch.argmax;  value = min / mean / lower median (SB_POLICY_*) over p[l][b][h] (fp32
+ *     [layers][batch][heads]) for l in [layer0, layers), as MMATextDecoderAgent's decision reduces p_choose.  The mean is a
+ *     float64 sum rounded once.  layers * heads <= SB_POLICY_MAX_VALUES; a stream with an unknown method or layer0 outside
+ *     [0, layers) gets {-1, NaN}. */
+#define SB_POLICY_MIN 0
+#define SB_POLICY_MEAN 1
+#define SB_POLICY_MEDIAN 2
+#define SB_POLICY_MAX_BLOCKED 4
+#define SB_POLICY_MAX_VALUES 4096
+#define SB_POLICY_CTL 6
+int sb_pchoose_ragged(const void* q_energy, int32_t q_rows, const void* k_energy, int32_t k_rows, const int32_t* q_lens,
+                      const int32_t* k_lens, float* p, int32_t batch, int32_t heads, float energy_bias, float temperature,
+                      sb_stream_t stream);
+int sb_policy_decide(const float* logits, int64_t ld, int32_t vocab, const int32_t* ctl, const float* p, int32_t layers,
+                     int32_t heads, int32_t batch, int32_t* out, sb_stream_t stream);
+
 /* small utilities */
 int sb_cast_f32_to_f16(const float* src, void* dst, int64_t n, sb_stream_t stream);
 int sb_fill_zero(void* dst, int64_t bytes, sb_stream_t stream);

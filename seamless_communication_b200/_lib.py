@@ -97,6 +97,8 @@ PROTOTYPES = {
     "sb_conv_post_tanh": [c_p, i32, i32, i32, c_p, i32, i32, c_p, f32, i32, c_p, i64, c_p],
     "sb_avgpool_time": [c_p, c_p, i32, i32, i32, i32, c_p],
     "sb_pchoose": [c_p, c_p, c_p, i32, i32, i32, f32, f32, c_p],
+    "sb_pchoose_ragged": [c_p, i32, c_p, i32, c_p, c_p, c_p, i32, i32, f32, f32, c_p],
+    "sb_policy_decide": [c_p, i64, i32, c_p, c_p, i32, i32, i32, c_p, c_p],
     "sb_cast_f32_to_f16": [c_p, c_p, i64, c_p],
     "sb_fill_zero": [c_p, i64, c_p],
 }

@@ -406,6 +406,50 @@ def token_timestamps(hist: torch.Tensor, slots: torch.Tensor, n_tok: torch.Tenso
     return starts
 
 
+POLICY_METHODS = {"min": 0, "mean": 1, "median": 2}  # SB_POLICY_MIN / _MEAN / _MEDIAN
+POLICY_MAX_BLOCKED, POLICY_CTL = 4, 6  # SB_POLICY_MAX_BLOCKED, SB_POLICY_CTL
+
+
+def policy_ctl(blocked, method: str, layer0: int, layers: int) -> list:
+    """One stream's row of sb_policy_decide's ctl: up to 4 blocked ids, the decision method and the first p_choose layer.
+    layer0 means what `p_choose[layer0:]` means in the single-stream decision: a negative one counts from the end (and
+    clamps at 0); one that leaves no layer raises, as the reduction of an empty slice does there."""
+    blocked = list(blocked)
+    if len(blocked) > POLICY_MAX_BLOCKED:
+        raise ValueError(f"at most {POLICY_MAX_BLOCKED} blocked ids, got {len(blocked)}")
+    if method not in POLICY_METHODS:
+        raise ValueError(f"`decision_method` must be 'min', 'mean' or 'median', but is '{method}' instead.")
+    first = range(layers)[layer0:]
+    if len(first) == 0:
+        raise ValueError(f"p_choose_start_layer {layer0} leaves none of the {layers} layers")
+    return blocked + [-1] * (POLICY_MAX_BLOCKED - len(blocked)) + [POLICY_METHODS[method], first.start]
+
+
+def pchoose_ragged(q: Seq, k: Seq, q_lens: torch.Tensor, k_lens: torch.Tensor, heads: int, energy_bias: float,
+                   temperature: float, out: torch.Tensor) -> torch.Tensor:
+    """out (B, heads) fp32 = p_choose of each stream's newest target position (q_lens - 1) against its last pooled source
+    position (k_lens - 1), from the q / k energies in sequence layout (sb_pchoose_ragged)."""
+    assert q.PH == 0 and k.PH == 0 and q.B == k.B and out.is_contiguous()
+    check(_lib.load().sb_pchoose_ragged(q.buf.data_ptr(), q.Tp, k.buf.data_ptr(), k.Tp, q_lens.data_ptr(), k_lens.data_ptr(),
+                                        out.data_ptr(), q.B, heads, energy_bias, temperature, _stream()), "sb_pchoose_ragged")
+    return out
+
+
+def policy_decide(logits: torch.Tensor, ctl: torch.Tensor, p: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """logits (B, >= V) fp32 with unit column stride, ctl (B, 6) int32 on the device (rows of policy_ctl), p (layers, B, heads)
+    fp32 -> (B, 2) int32: the token and the float bits of the decision value of each stream (sb_policy_decide)."""
+    B, V = logits.shape
+    layers, _, heads = p.shape
+    assert logits.dtype == torch.float32 and p.dtype == torch.float32, "sb_policy_decide reads fp32 logits and p_choose"
+    assert logits.stride(1) == 1 and p.is_contiguous() and p.shape[1] == B
+    assert ctl.is_contiguous() and ctl.dtype == torch.int32 and tuple(ctl.shape) == (B, POLICY_CTL)
+    if out is None:
+        out = torch.empty((B, 2), dtype=torch.int32, device=logits.device)
+    check(_lib.load().sb_policy_decide(logits.data_ptr(), logits.stride(0), V, ctl.data_ptr(), p.data_ptr(), layers, heads, B,
+                                       out.data_ptr(), _stream()), "sb_policy_decide")
+    return out
+
+
 def embed_seq(ids: torch.Tensor, embed, pos, scale, dim) -> torch.Tensor:
     lib = _lib.load()
     R, L = ids.shape

@@ -33,6 +33,7 @@ class MMATextDecoderPolicy:
         self.target_indices: List[int] = []
         self.target_finished = False
         self.ngram_block_count = 0
+        self._call = None
 
     def _decide(self, p_choose: torch.Tensor) -> float:
         last = p_choose[self.start_layer:, :, -1, -1]  # (layers, heads) (:233-243)
@@ -42,16 +43,15 @@ class MMATextDecoderPolicy:
             return float(last.mean())
         return float(last.median())
 
-    def _run_decoder(self, encoder_output, pred: List[int], source_finished: bool) -> Tuple[int, float]:
+    def _run_decoder(self, encoder_output, pred: List[int]) -> Tuple[int, float]:
         """run_decoder (:205-243).  The reference feeds only the newest token and keeps an IncrementalStateBag per policy
         call; this engine re-runs the (short) prefix, which yields the same last-position outputs."""
         ids = torch.tensor([self.prefix + self.target_indices + pred], dtype=torch.int64)
         dec, p_choose = self.model.decode(ids, encoder_output)
         logits = self.model.project(dec[:, -1:])[0, -1].float().clone()
-        if self.block_ngrams and source_finished:
-            blocked = (self.target_indices + pred)[-4:]
-            if blocked:
-                logits[blocked] = float("-inf")
+        blocked = self.blocked_ids()
+        if blocked:
+            logits[blocked] = float("-inf")
         return int(logits.argmax().item()), self._decide(p_choose)
 
     def _blocked_ngrams(self) -> Optional[Set[str]]:  # get_blocked_ngrams (:260-274)
@@ -82,43 +82,81 @@ class MMATextDecoderPolicy:
                 blocked.add(str(all_indices[-n:]))
         return False
 
-    @torch.inference_mode()
-    def policy(self, encoder_output: torch.Tensor, source_finished: bool) -> Tuple[List[int], bool]:
-        """One call of the agent's policy (:304-387).  Returns (tokens written by this call, finished); ([], False) is a
-        READ.  As under SimulEval, call again with the same source after a WRITE; feed more source after a READ."""
-        source_len = 0 if encoder_output is None else int(encoder_output.shape[1])
+    # -------------------------------------------------------------------------- one policy call, a token at a time
+    # policy() below is begin() followed by decoder runs fed to step() until it returns.  A multi-stream driver
+    # (StreamingS2STBatch) calls the same three methods, so that every stream takes exactly the decisions policy() takes,
+    # while the decoder runs of many streams go through the device as one batch.
+    def begin(self, source_len: int, source_finished: bool) -> Optional[Tuple[List[int], bool]]:
+        """Starts one policy call on `source_len` encoder frames.  Returns the call's result when it ends without running
+        the decoder; otherwise None, and the call continues with step()."""
+        self._call = None
         if source_len == 0:
             return [], False
         if source_len < self.min_starting_wait and not source_finished:
             return [], False
         if self.target_finished:
             return [], True
-        max_len = self.max_len_a * source_len + self.max_len_b
-        pred: List[int] = []
-        finished = False
-        blocked = self._blocked_ngrams()
-        while True:
-            index, prob = self._run_decoder(encoder_output, pred, source_finished)
-            if self.no_early_stop and not source_finished and (prob < self.threshold or index == self.eos):
-                if prob == 1.0:
-                    pred = []
-                break
-            if self._maybe_block(pred, blocked, index, source_finished):
-                break
-            if finished or index == self.eos or len(self.target_indices) + len(pred) > max_len:
-                finished = True
-                break
-            if prob < self.threshold and not source_finished:
-                break  # READ
-            if len(self.target_indices) + len(pred) >= max_len or len(pred) >= self.max_writes:
-                break
-            pred.append(index)
+        self._call = dict(max_len=self.max_len_a * source_len + self.max_len_b, pred=[], finished=False,
+                          blocked=self._blocked_ngrams(), source_finished=source_finished)
+        return None
+
+    @property
+    def pending(self) -> List[int]:
+        """Tokens written so far by the current call (not yet in target_indices)."""
+        return self._call["pred"]
+
+    def decoder_ids(self) -> List[int]:
+        """The token prefix of the current call's next decoder run."""
+        return self.prefix + self.target_indices + self._call["pred"]
+
+    def blocked_ids(self) -> List[int]:
+        """Token ids set to -inf before the argmax of the current call's next decoder run (the `block_ngrams and
+        source_finished` rule of run_decoder, at most 4)."""
+        if self.block_ngrams and self._call["source_finished"]:
+            return (self.target_indices + self._call["pred"])[-4:]
+        return []
+
+    def step(self, index: int, prob: float) -> Optional[Tuple[List[int], bool]]:
+        """Feeds the newest position's token and decision value of one decoder run (:344-369).  Returns the call's result
+        (as policy() does) when the call ends, or None when it wants another decoder run."""
+        c = self._call
+        pred, max_len, source_finished = c["pred"], c["max_len"], c["source_finished"]
+        if self.no_early_stop and not source_finished and (prob < self.threshold or index == self.eos):
+            if prob == 1.0:
+                c["pred"] = pred = []
+            return self._end()
+        if self._maybe_block(pred, c["blocked"], index, source_finished):
+            return self._end()
+        if c["finished"] or index == self.eos or len(self.target_indices) + len(pred) > max_len:
+            c["finished"] = True
+            return self._end()
+        if prob < self.threshold and not source_finished:
+            return self._end()  # READ
+        if len(self.target_indices) + len(pred) >= max_len or len(pred) >= self.max_writes:
+            return self._end()
+        pred.append(index)
+        return None
+
+    def _end(self) -> Tuple[List[int], bool]:
+        c, self._call = self._call, None
+        pred, finished = c["pred"], c["finished"]
         self.target_indices += pred
         if len(pred) > 0 or finished:
             # the reference re-checks the budget with `states.target_indices + pred_indices` AFTER the append above, i.e.
             # it counts this call's tokens twice (:374-377); mirrored
-            finished = finished or len(self.target_indices) + len(pred) > max_len
+            finished = finished or len(self.target_indices) + len(pred) > c["max_len"]
             self.ngram_block_count = 0
             self.target_finished = finished
             return pred, finished
         return [], False
+
+    @torch.inference_mode()
+    def policy(self, encoder_output: torch.Tensor, source_finished: bool) -> Tuple[List[int], bool]:
+        """One call of the agent's policy (:304-387).  Returns (tokens written by this call, finished); ([], False) is a
+        READ.  As under SimulEval, call again with the same source after a WRITE; feed more source after a READ."""
+        source_len = 0 if encoder_output is None else int(encoder_output.shape[1])
+        done = self.begin(source_len, source_finished)
+        while done is None:
+            index, prob = self._run_decoder(encoder_output, self.pending)
+            done = self.step(index, prob)
+        return done
