@@ -282,7 +282,9 @@ int sb_decode_cross_attn_weights(const float* q_partials, int32_t splits, int64_
                                  int64_t kv_ld, const int32_t* enc_lens, int32_t s_enc, const int32_t* step_ptr, float* hist,
                                  int32_t rows, int32_t beam, int32_t heads, sb_stream_t stream);
 /* per row: log-softmax statistics and the top-K candidates of an fp32 logit row.
- *   cand_val [rows][K] = lprob, cand_idx [rows][K]; eos_lprob[rows] = lprob of eos; pad is never a candidate. */
+ *   cand_val [rows][K] = lprob, cand_idx [rows][K] in (lprob desc, id asc) order, (-inf, 0) past the last candidate;
+ *   eos_lprob[rows] = lprob of eos; pad is never a candidate; unk's candidate value is its logit - unk_penalty.
+ * SB_EINVAL unless logits is 16-byte aligned, ld a multiple of 4 and 0 <= eos_idx < vocab (all four entry points). */
 int sb_logits_topk(const float* logits, int64_t ld, int32_t rows, int32_t vocab, int32_t pad_idx, int32_t eos_idx,
                    int32_t unk_idx, float unk_penalty, int32_t K, float* cand_val, int32_t* cand_idx, float* eos_lprob,
                    sb_stream_t stream);
@@ -290,6 +292,7 @@ int sb_logits_topk(const float* logits, int64_t ld, int32_t rows, int32_t vocab,
 /* Same contract as sb_logits_topk, for logits written by sb_gemm with `tile_stats`: the log-sum-exp comes from the tile
  * statistics and only the tiles whose maximum reaches the (K+2)-th largest tile maximum are read back (a lower bound of the
  * K-th best candidate even if PAD and UNK head two of them), i.e. ~K x 512 B per row instead of two passes over the row.
+ * Vocabularies of fewer than K+2 tiles of 128 run sb_logits_topk's kernel instead (the statistics are not read).
  * Replaces log_softmax + topk over the vocabulary (fairseq2.cpp:1463-1516) without the 164 MB round trips per step. */
 int sb_logits_topk_tiles(const float* logits, int64_t ld, const float* tile_stats, int32_t rows, int32_t vocab, int32_t pad_idx,
                          int32_t eos_idx, int32_t unk_idx, float unk_penalty, int32_t K, float* cand_val, int32_t* cand_idx,

@@ -476,7 +476,10 @@ __global__ void __launch_bounds__(256) decode_cross_attn_shared_kernel(const flo
 //   pass 1: online max / sum-exp over the raw logits, plus each thread's single best candidate;
 //           tau = K-th largest of the per-thread bests is a lower bound of the K-th largest candidate overall;
 //   pass 2: every candidate >= tau (a few dozen at most, barring massive ties) is appended to a shared list;
-//   a single warp then extracts the top K in (value desc, index asc) order.
+//   a single warp then extracts the top K in (value desc, index asc) order, and fills the row with (-inf, 0) past the
+//   last candidate.
+// The list holds TK_CAP candidates: with more than that many at or above tau (more than TK_CAP tokens tied at the K-th
+// value) it keeps those that arrive first, and which of the tied tokens are returned is unspecified.
 constexpr int TK_MAX = 16;
 constexpr int TK_THREADS = 512;
 constexpr int TK_CAP = 2048;
@@ -510,6 +513,59 @@ __device__ __forceinline__ float tk_cand_b(float x, int i, int pad_idx, int unk_
   return tk_cand(x, i, pad_idx, unk_idx, unk_penalty);
 }
 
+// Run by one warp: the K-th largest of the NT per-thread best candidates s_best[0 .. NT) (each lane owns NT / 32 of
+// them).  Every per-thread best is a candidate, so at least K candidates reach it; -inf when fewer than K threads saw one.
+template <int NT>
+__device__ __forceinline__ float tk_kth_best(const float* s_best, int K) {
+  const int lane = threadIdx.x & 31;
+  float loc[NT / 32];
+#pragma unroll
+  for (int i = 0; i < NT / 32; ++i) loc[i] = s_best[lane * (NT / 32) + i];
+  float tau = -INFINITY;
+  for (int round = 0; round < K; ++round) {
+    float lm = -INFINITY; int li = 0;
+#pragma unroll
+    for (int i = 0; i < NT / 32; ++i) if (loc[i] > lm) { lm = loc[i]; li = i; }
+    const float wm = warp_max(lm);
+    tau = wm;
+    // the first lane holding the maximum removes one copy
+    const unsigned ball = __ballot_sync(0xffffffffu, lm == wm);
+    if (lane == __ffs(ball) - 1) {
+#pragma unroll
+      for (int i = 0; i < NT / 32; ++i) if (i == li) loc[i] = -INFINITY;
+    }
+  }
+  return tau;
+}
+
+// Run by one warp: the top K of the candidate list s_cv / s_ci [0 .. n) in (value desc, index asc) order as lprobs
+// (value - lse) into row r of cand_val / cand_idx, then (-inf, 0) once the list is exhausted.  Consumes the list.
+__device__ __forceinline__ void tk_extract(float* s_cv, const int* s_ci, int n, int K, float lse, long long r,
+                                           float* __restrict__ cand_val, int* __restrict__ cand_idx) {
+  const int lane = threadIdx.x & 31;
+  for (int round = 0; round < K; ++round) {
+    float bv = -INFINITY; int bi = 0x7fffffff, bs = -1;
+    for (int j = lane; j < n; j += 32) {
+      const float v = s_cv[j]; const int id = s_ci[j];
+      if (v > bv || (v == bv && id < bi)) { bv = v; bi = id; bs = j; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float v2 = __shfl_xor_sync(0xffffffffu, bv, o);
+      const int i2 = __shfl_xor_sync(0xffffffffu, bi, o);
+      const int s2 = __shfl_xor_sync(0xffffffffu, bs, o);
+      if (v2 > bv || (v2 == bv && i2 < bi)) { bv = v2; bi = i2; bs = s2; }
+    }
+    if (lane == 0) {
+      const bool ok = bv > -INFINITY;  // else every candidate is taken (marked -inf)
+      cand_val[r * K + round] = ok ? bv - lse : -INFINITY;
+      cand_idx[r * K + round] = ok ? bi : 0;
+      if (ok) s_cv[bs] = -INFINITY;
+    }
+    __syncwarp();
+  }
+}
+
 // BAN: row r's banned ids are ban_ids[r * ban_ld .. + ban_n[r]] (dynamic shared memory: the vocabulary bitmap)
 template <bool BAN>
 __global__ void __launch_bounds__(TK_THREADS) logits_topk_kernel(const float* __restrict__ logits, long long ld, int vocab,
@@ -537,16 +593,17 @@ __global__ void __launch_bounds__(TK_THREADS) logits_topk_kernel(const float* __
     const float xs[4] = {v.x, v.y, v.z, v.w};
     const float m4 = fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w));
     if (m4 > mx) { sum *= __expf(mx - m4); mx = m4; }
+    const float ms = mx == -INFINITY ? 0.f : mx;  // all four are -inf then: exp(-inf - -inf) would be NaN
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
-      sum += __expf(xs[e] - mx);
+      sum += __expf(xs[e] - ms);
       best = fmaxf(best, tk_cand_b<BAN>(xs[e], 4 * i + e, pad_idx, unk_idx, unk_penalty, tk_bits));
     }
   }
   for (int i = 4 * nvec + threadIdx.x; i < vocab; i += TK_THREADS) {
     const float x = row[i];
     if (x > mx) { sum *= __expf(mx - x); mx = x; }
-    sum += __expf(x - mx);
+    sum += __expf(x - (mx == -INFINITY ? 0.f : mx));
     best = fmaxf(best, tk_cand_b<BAN>(x, i, pad_idx, unk_idx, unk_penalty, tk_bits));
   }
   s_best[threadIdx.x] = best;
@@ -566,24 +623,7 @@ __global__ void __launch_bounds__(TK_THREADS) logits_topk_kernel(const float* __
       s_lse = M + logf(S);
       eos_lprob[r] = (BAN && tk_banned(tk_bits, eos_idx)) ? -INFINITY : row[eos_idx] - (M + logf(S));
     }
-    // K-th largest of the 512 per-thread bests: each lane owns 16 of them
-    float loc[TK_THREADS / 32];
-#pragma unroll
-    for (int i = 0; i < TK_THREADS / 32; ++i) loc[i] = s_best[lane * (TK_THREADS / 32) + i];
-    float tau = -INFINITY;
-    for (int round = 0; round < K; ++round) {
-      float lm = -INFINITY; int li = 0;
-#pragma unroll
-      for (int i = 0; i < TK_THREADS / 32; ++i) if (loc[i] > lm) { lm = loc[i]; li = i; }
-      const float wm = warp_max(lm);
-      tau = wm;
-      // the first lane holding the maximum removes one copy
-      const unsigned ball = __ballot_sync(0xffffffffu, lm == wm);
-      if (lane == __ffs(ball) - 1) {
-#pragma unroll
-        for (int i = 0; i < TK_THREADS / 32; ++i) if (i == li) loc[i] = -INFINITY;
-      }
-    }
+    const float tau = tk_kth_best<TK_THREADS>(s_best, K);
     if (lane == 0) s_tau = tau;
   }
   __syncthreads();
@@ -610,29 +650,7 @@ __global__ void __launch_bounds__(TK_THREADS) logits_topk_kernel(const float* __
   }
   __syncthreads();
   // ---- top-K of the candidate list, one warp
-  if (warp == 0) {
-    const int n = min(s_count, TK_CAP);
-    for (int round = 0; round < K; ++round) {
-      float bv = -INFINITY; int bi = 0x7fffffff, bs = -1;
-      for (int j = lane; j < n; j += 32) {
-        const float v = s_cv[j]; const int id = s_ci[j];
-        if (v > bv || (v == bv && id < bi)) { bv = v; bi = id; bs = j; }
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const float v2 = __shfl_xor_sync(0xffffffffu, bv, o);
-        const int i2 = __shfl_xor_sync(0xffffffffu, bi, o);
-        const int s2 = __shfl_xor_sync(0xffffffffu, bs, o);
-        if (v2 > bv || (v2 == bv && i2 < bi)) { bv = v2; bi = i2; bs = s2; }
-      }
-      if (lane == 0) {
-        cand_val[(long long)r * K + round] = bs >= 0 ? bv - lse : -INFINITY;
-        cand_idx[(long long)r * K + round] = bs >= 0 ? bi : 0;
-        if (bs >= 0) s_cv[bs] = -INFINITY;
-      }
-      __syncwarp();
-    }
-  }
+  if (warp == 0) tk_extract(s_cv, s_ci, min(s_count, TK_CAP), K, lse, r, cand_val, cand_idx);
 }
 
 // Top-K from per-tile statistics (written by the projection GEMM's epilogue, sb_gemm tile_stats): one CTA per row.
@@ -641,9 +659,15 @@ __global__ void __launch_bounds__(TK_THREADS) logits_topk_kernel(const float* __
 //      candidate and the UNK penalty can push one more below);
 //   3. only the tiles whose maximum reaches tau are read back (one warp per tile, 512 B) and their elements >= tau collected;
 //   4. the same (value desc, index asc) extraction as logits_topk_kernel.
+// A negative UNK penalty lifts UNK above its raw value: UNK's tile then counts with max(tile maximum, UNK's candidate
+// value), so that the tile is read whenever UNK reaches tau and every counted maximum is still reached by a token.
 // BAN: a tile whose maximum is a banned token ("tainted") takes no part in step 2, so tau is the (K+2)-th largest maximum
 // of the untainted tiles, each of which is reached by a token that is not banned: the bound holds whatever the number of
 // bans, and the candidate list does not grow with it.  Step 3 still reads tainted tiles and skips banned tokens.
+// The wrappers need at least K+2 tiles (smaller vocabularies go to logits_topk_kernel).  When fewer than K+2 tiles are
+// untainted, step 2 ends at tau = -inf, and tau is then taken from the per-thread best candidates of the whole row as in
+// logits_topk_kernel: a full read of the row, but a candidate list that stays short.  The limit on exact ties at the
+// K-th value is logits_topk_kernel's.
 constexpr int TKT_THREADS = 256;
 constexpr int TKT_TILE = 128;
 
@@ -700,6 +724,8 @@ __global__ void __launch_bounds__(TKT_THREADS) logits_topk_tiles_kernel(const fl
     for (int i = 0; i < nwarp; ++i) S += s_red[i];
     s_lse = M + logf(S);
     eos_lprob[r] = (BAN && tk_banned(bits, eos_idx)) ? -INFINITY : row[eos_idx] - (M + logf(S));
+    if (unk_penalty < 0.f && unk_idx >= 0 && unk_idx < vocab && unk_idx != pad_idx && !(BAN && tk_banned(bits, unk_idx)))
+      tk_sm[unk_idx / TKT_TILE] = fmaxf(tk_sm[unk_idx / TKT_TILE], row[unk_idx] - unk_penalty);
   }
   __syncthreads();
   // ---- 2. tau = (K+2)-th largest tile maximum (block-wide arg-max, K+2 rounds; the found tile is marked by negating into
@@ -743,6 +769,25 @@ __global__ void __launch_bounds__(TKT_THREADS) logits_topk_tiles_kernel(const fl
     __syncthreads();
     tau = s_tau;
   }
+  if (tau == -INFINITY) {  // block-uniform: fewer than K+2 untainted tiles; s_cv is free until step 3
+    float best = -INFINITY;
+    for (int i = threadIdx.x; i < (vocab >> 2); i += TKT_THREADS) {
+      const float4 v = *reinterpret_cast<const float4*>(row + 4 * i);
+      const float xs[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) best = fmaxf(best, tk_cand_b<BAN>(xs[e], 4 * i + e, pad_idx, unk_idx, unk_penalty, bits));
+    }
+    for (int i = (vocab & ~3) + threadIdx.x; i < vocab; i += TKT_THREADS)
+      best = fmaxf(best, tk_cand_b<BAN>(row[i], i, pad_idx, unk_idx, unk_penalty, bits));
+    s_cv[threadIdx.x] = best;
+    __syncthreads();
+    if (warp == 0) {
+      const float t = tk_kth_best<TKT_THREADS>(s_cv, K);
+      if (lane == 0) s_tau = t;
+    }
+    __syncthreads();
+    tau = s_tau;
+  }
   // ---- 3. gather candidates >= tau from the tiles that can hold one
   for (int t = warp; t < n_tiles; t += nwarp) {
     if (!(tk_sm[t] >= tau)) continue;  // warp-uniform
@@ -767,30 +812,7 @@ __global__ void __launch_bounds__(TKT_THREADS) logits_topk_tiles_kernel(const fl
   }
   __syncthreads();
   // ---- 4. top-K of the candidate list, one warp
-  if (warp == 0) {
-    const float lse = s_lse;
-    const int n = min(s_count, TK_CAP);
-    for (int round = 0; round < K; ++round) {
-      float bv = -INFINITY; int bi = 0x7fffffff, bs = -1;
-      for (int j = lane; j < n; j += 32) {
-        const float v = s_cv[j]; const int id = s_ci[j];
-        if (v > bv || (v == bv && id < bi)) { bv = v; bi = id; bs = j; }
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const float v2 = __shfl_xor_sync(0xffffffffu, bv, o);
-        const int i2 = __shfl_xor_sync(0xffffffffu, bi, o);
-        const int s2 = __shfl_xor_sync(0xffffffffu, bs, o);
-        if (v2 > bv || (v2 == bv && i2 < bi)) { bv = v2; bi = i2; bs = s2; }
-      }
-      if (lane == 0) {
-        cand_val[(long long)r * K + round] = bs >= 0 ? bv - lse : -INFINITY;
-        cand_idx[(long long)r * K + round] = bs >= 0 ? bi : 0;
-        if (bs >= 0) s_cv[bs] = -INFINITY;
-      }
-      __syncwarp();
-    }
-  }
+  if (warp == 0) tk_extract(s_cv, s_ci, min(s_count, TK_CAP), K, s_lse, r, cand_val, cand_idx);
 }
 
 // ------------------------------------------------------------------------------------------- beam bookkeeping
@@ -1134,18 +1156,33 @@ extern "C" int sb_decode_cross_attn_weights(const float* q_partials, int32_t spl
   return SB_OK;
 }
 
+// logits_topk_kernel<BAN> for the two-pass entry points, and for the tile entry points below K+2 tiles (at most 2176
+// tokens: the statistics are not needed there)
+template <bool BAN>
+static int topk_two_pass(const float* logits, int64_t ld, int32_t rows, int32_t vocab, int32_t pad_idx, int32_t eos_idx,
+                         int32_t unk_idx, float unk_penalty, int32_t K, float* cand_val, int32_t* cand_idx, float* eos_lprob,
+                         const int32_t* ban_ids, const int32_t* ban_n, int32_t ban_ld, sb_stream_t stream) {
+  using namespace sb;
+  const size_t smem = BAN ? (size_t)(vocab + 31) / 32 * sizeof(unsigned) : 0;
+  if (BAN) SB_CUDA_OK(allow_dynamic_smem(logits_topk_kernel<BAN>, smem));
+  SB_CUDA_OK(prefer_shared((logits_topk_kernel<BAN>)));
+  SB_CUDA_OK(launch_k(logits_topk_kernel<BAN>, dim3(rows), dim3(TK_THREADS), smem, (cudaStream_t)stream, logits, (long long)ld,
+                       (int)vocab, (int)pad_idx, (int)eos_idx, (int)unk_idx, unk_penalty, (int)K, cand_val, (int*)cand_idx,
+                       eos_lprob, (const int*)ban_ids, (const int*)ban_n, (int)ban_ld));
+  count_launch();
+  return SB_OK;
+}
+
 extern "C" int sb_logits_topk(const float* logits, int64_t ld, int32_t rows, int32_t vocab, int32_t pad_idx, int32_t eos_idx,
                               int32_t unk_idx, float unk_penalty, int32_t K, float* cand_val, int32_t* cand_idx,
                               float* eos_lprob, sb_stream_t stream) {
   using namespace sb;
   SB_REQUIRE(logits && cand_val && cand_idx && eos_lprob && rows > 0 && vocab > 0, SB_EINVAL, "sb_logits_topk: bad args");
   SB_REQUIRE(K > 0 && K <= TK_MAX, SB_ENOSUP, "sb_logits_topk: K=%d unsupported (<= %d)", K, TK_MAX);
-  SB_CUDA_OK(prefer_shared((logits_topk_kernel<false>)));
-  SB_CUDA_OK(launch_k(logits_topk_kernel<false>, dim3(rows), dim3(TK_THREADS), 0, (cudaStream_t)stream, logits, (long long)ld,
-                       (int)vocab, (int)pad_idx, (int)eos_idx, (int)unk_idx, unk_penalty, (int)K, cand_val, (int*)cand_idx,
-                       eos_lprob, (const int*)nullptr, (const int*)nullptr, 0));
-  count_launch();
-  return SB_OK;
+  SB_REQUIRE(ld % 4 == 0 && ((uintptr_t)logits % 16) == 0, SB_EINVAL, "sb_logits_topk: logits must be 16-byte aligned rows");
+  SB_REQUIRE(eos_idx >= 0 && eos_idx < vocab, SB_EINVAL, "sb_logits_topk: eos_idx %d outside the vocabulary", eos_idx);
+  return topk_two_pass<false>(logits, ld, rows, vocab, pad_idx, eos_idx, unk_idx, unk_penalty, K, cand_val, cand_idx, eos_lprob,
+                              nullptr, nullptr, 0, stream);
 }
 
 extern "C" int sb_logits_topk_ban(const float* logits, int64_t ld, int32_t rows, int32_t vocab, int32_t pad_idx, int32_t eos_idx,
@@ -1156,15 +1193,12 @@ extern "C" int sb_logits_topk_ban(const float* logits, int64_t ld, int32_t rows,
   SB_REQUIRE(logits && cand_val && cand_idx && eos_lprob && ban_ids && ban_n && rows > 0 && vocab > 0 && ban_ld > 0, SB_EINVAL,
              "sb_logits_topk_ban: bad args");
   SB_REQUIRE(K > 0 && K <= TK_MAX, SB_ENOSUP, "sb_logits_topk_ban: K=%d unsupported (<= %d)", K, TK_MAX);
-  const size_t smem = (size_t)(vocab + 31) / 32 * sizeof(unsigned);
-  SB_REQUIRE(smem <= 160 * 1024, SB_ENOSUP, "sb_logits_topk_ban: vocabulary of %d too large", vocab);
-  SB_CUDA_OK(allow_dynamic_smem(logits_topk_kernel<true>, smem));
-  SB_CUDA_OK(prefer_shared((logits_topk_kernel<true>)));
-  SB_CUDA_OK(launch_k(logits_topk_kernel<true>, dim3(rows), dim3(TK_THREADS), smem, (cudaStream_t)stream, logits, (long long)ld,
-                       (int)vocab, (int)pad_idx, (int)eos_idx, (int)unk_idx, unk_penalty, (int)K, cand_val, (int*)cand_idx,
-                       eos_lprob, (const int*)ban_ids, (const int*)ban_n, (int)ban_ld));
-  count_launch();
-  return SB_OK;
+  SB_REQUIRE(ld % 4 == 0 && ((uintptr_t)logits % 16) == 0, SB_EINVAL, "sb_logits_topk_ban: logits must be 16-byte aligned rows");
+  SB_REQUIRE(eos_idx >= 0 && eos_idx < vocab, SB_EINVAL, "sb_logits_topk_ban: eos_idx %d outside the vocabulary", eos_idx);
+  SB_REQUIRE((size_t)(vocab + 31) / 32 * sizeof(unsigned) <= 160 * 1024, SB_ENOSUP, "sb_logits_topk_ban: vocabulary of %d too large",
+             vocab);
+  return topk_two_pass<true>(logits, ld, rows, vocab, pad_idx, eos_idx, unk_idx, unk_penalty, K, cand_val, cand_idx, eos_lprob,
+                             ban_ids, ban_n, ban_ld, stream);
 }
 
 extern "C" int sb_logits_topk_tiles(const float* logits, int64_t ld, const float* tile_stats, int32_t rows, int32_t vocab,
@@ -1174,7 +1208,11 @@ extern "C" int sb_logits_topk_tiles(const float* logits, int64_t ld, const float
   SB_REQUIRE(logits && tile_stats && cand_val && cand_idx && eos_lprob && rows > 0 && vocab > 0, SB_EINVAL, "sb_logits_topk_tiles: bad args");
   SB_REQUIRE(K > 0 && K <= TK_MAX, SB_ENOSUP, "sb_logits_topk_tiles: K=%d unsupported (<= %d)", K, TK_MAX);
   SB_REQUIRE(ld % 4 == 0 && ((uintptr_t)logits % 16) == 0, SB_EINVAL, "sb_logits_topk_tiles: logits must be 16-byte aligned rows");
+  SB_REQUIRE(eos_idx >= 0 && eos_idx < vocab, SB_EINVAL, "sb_logits_topk_tiles: eos_idx %d outside the vocabulary", eos_idx);
   const int n_tiles = (vocab + TKT_TILE - 1) / TKT_TILE;
+  if (n_tiles < K + 2)
+    return topk_two_pass<false>(logits, ld, rows, vocab, pad_idx, eos_idx, unk_idx, unk_penalty, K, cand_val, cand_idx, eos_lprob,
+                                nullptr, nullptr, 0, stream);
   const size_t smem = (size_t)2 * n_tiles * sizeof(float);
   SB_REQUIRE(smem <= 40 * 1024, SB_ENOSUP, "sb_logits_topk_tiles: vocabulary of %d too large", vocab);
   SB_CUDA_OK(prefer_shared((logits_topk_tiles_kernel<false>)));
@@ -1194,7 +1232,11 @@ extern "C" int sb_logits_topk_tiles_ban(const float* logits, int64_t ld, const f
              SB_EINVAL, "sb_logits_topk_tiles_ban: bad args");
   SB_REQUIRE(K > 0 && K <= TK_MAX, SB_ENOSUP, "sb_logits_topk_tiles_ban: K=%d unsupported (<= %d)", K, TK_MAX);
   SB_REQUIRE(ld % 4 == 0 && ((uintptr_t)logits % 16) == 0, SB_EINVAL, "sb_logits_topk_tiles_ban: logits must be 16-byte aligned rows");
+  SB_REQUIRE(eos_idx >= 0 && eos_idx < vocab, SB_EINVAL, "sb_logits_topk_tiles_ban: eos_idx %d outside the vocabulary", eos_idx);
   const int n_tiles = (vocab + TKT_TILE - 1) / TKT_TILE;
+  if (n_tiles < K + 2)
+    return topk_two_pass<true>(logits, ld, rows, vocab, pad_idx, eos_idx, unk_idx, unk_penalty, K, cand_val, cand_idx, eos_lprob,
+                               ban_ids, ban_n, ban_ld, stream);
   const size_t smem = (size_t)2 * n_tiles * sizeof(float) + (size_t)(vocab + 31) / 32 * sizeof(unsigned);
   SB_REQUIRE((size_t)2 * n_tiles * sizeof(float) <= 40 * 1024, SB_ENOSUP, "sb_logits_topk_tiles_ban: vocabulary of %d too large", vocab);
   SB_CUDA_OK(allow_dynamic_smem(logits_topk_tiles_kernel<true>, smem));

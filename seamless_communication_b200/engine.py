@@ -32,6 +32,14 @@ I32 = torch.int32
 _CAPTURE_LOCK = threading.Lock()
 
 
+def _capture_stream() -> Optional[torch.cuda.Stream]:
+    """The stream a step graph is captured on: the calling thread's own stream when it has one (a LanePool lane), else
+    torch's capture stream.  torch hands its pool's 32 streams out round-robin, so a capture stream shared by every thread
+    can be another lane's stream, and that lane's work would then run inside the capture."""
+    cur = torch.cuda.current_stream()
+    return None if cur == torch.cuda.default_stream(cur.device) else cur
+
+
 def sinusoid_table(max_len: int, dim: int, legacy_pad_idx: int = 1) -> torch.Tensor:
     """SinusoidalPositionEncoder table ([fs2-recall], oracle/ASSUMPTIONS.md #4; slice mirrored fairseq2.cpp:900-915)."""
     half = dim // 2
@@ -563,11 +571,11 @@ class UnitYEngine:
         torch.cuda.current_stream().wait_stream(s)
         n0 = ops.launch_count()
         st["g_fwd"] = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(st["g_fwd"], capture_error_mode="thread_local"):
+        with torch.cuda.graph(st["g_fwd"], stream=_capture_stream(), capture_error_mode="thread_local"):
             self._decoder_step_forward(st)
         n1 = ops.launch_count()
         st["g_sel"] = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(st["g_sel"], capture_error_mode="thread_local"):
+        with torch.cuda.graph(st["g_sel"], stream=_capture_stream(), capture_error_mode="thread_local"):
             self._decoder_step_select(st)
         st["n_fwd"], st["n_sel"] = n1 - n0, ops.launch_count() - n1
 
@@ -582,7 +590,7 @@ class UnitYEngine:
             torch.cuda.current_stream().wait_stream(s)
             n0 = ops.launch_count()
             st["g_sel_ban"] = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(st["g_sel_ban"], capture_error_mode="thread_local"):
+            with torch.cuda.graph(st["g_sel_ban"], stream=_capture_stream(), capture_error_mode="thread_local"):
                 self._decoder_step_select(st, ban=True)
             st["n_sel_ban"] = ops.launch_count() - n0
 
@@ -597,7 +605,7 @@ class UnitYEngine:
             torch.cuda.current_stream().wait_stream(s)
             n0 = ops.launch_count()
             st["g_fwd_attn"] = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(st["g_fwd_attn"], capture_error_mode="thread_local"):
+            with torch.cuda.graph(st["g_fwd_attn"], stream=_capture_stream(), capture_error_mode="thread_local"):
                 self._decoder_step_forward(st, record=True)
             st["n_fwd_attn"] = ops.launch_count() - n0
 

@@ -640,17 +640,19 @@ def test_full_width_properties_permutation_padding_determinism(small, ops):
 
 
 # ------------------------------------------------------------------------------------------------ BASELINE width (config 3)
-def _replay_search_on_logits(eng, trace, prefix, beam, V, len_penalty=1.0, min_len=1):
-    """Drive the INTEGER half of the search (sb_logits_topk -> sb_beam_step -> sb_step_advance, exactly as
-    engine._decoder_step_select does) with the oracle's fp32 logits, step by step, for one sentence.  Returns what the
-    device decided at every step: (parent beam indices, next tokens), and the finished hypotheses.  `min_len` is the
-    search's min_seq_len (EOS is blocked before that step)."""
+def _replay_search_on_logits(cfg, trace, prefix, beam, V, len_penalty=1.0, min_len=1, tiles=False, unk_penalty=0.0):
+    """Drive the INTEGER half of the search (top-K -> sb_beam_step -> sb_step_advance, exactly as
+    engine._decoder_step_select does) with the oracle's fp32 logits, step by step, for one sentence of the search over
+    `cfg`'s text vocabulary.  Returns what the device decided at every step: (parent beam indices, next tokens), and the
+    finished hypotheses.  `min_len` is the search's min_seq_len (EOS is blocked before that step); `tiles` selects
+    sb_logits_topk_tiles on the tile statistics of the logits instead of the two-pass sb_logits_topk."""
     import ctypes as Ct
     from seamless_communication_b200 import _lib
     from seamless_communication_b200._lib import BeamDesc, check
+    from test_mintox import _tile_stats
     lib = _lib.load()
     st = torch.cuda.current_stream().cuda_stream
-    ML, P, R, c = trace["max_len"], len(prefix), beam, eng.cfg
+    ML, P, R, c = trace["max_len"], len(prefix), beam, cfg
     K = min(2 * beam + 1, 16)
     ld = (V + 7) // 8 * 8
     i32 = dict(dtype=torch.int32, device=dev)
@@ -676,8 +678,13 @@ def _replay_search_on_logits(eng, trace, prefix, beam, V, len_penalty=1.0, min_l
         pos = P - 1 + s
         assert seqs[:, pos].tolist() == trace["inputs"][s].tolist(), f"step {s}: device rows feed other tokens than the oracle's"
         logits[:, :V] = lg.to(dev)
-        check(lib.sb_logits_topk(logits.data_ptr(), ld, R, V, c.text_pad, c.text_eos, c.text_unk, 0.0, K, cv.data_ptr(), ci.data_ptr(),
-                                 el.data_ptr(), st))
+        if tiles:
+            stats = _tile_stats(logits, V)
+            check(lib.sb_logits_topk_tiles(logits.data_ptr(), ld, stats.data_ptr(), R, V, c.text_pad, c.text_eos, c.text_unk, unk_penalty,
+                                           K, cv.data_ptr(), ci.data_ptr(), el.data_ptr(), st))
+        else:
+            check(lib.sb_logits_topk(logits.data_ptr(), ld, R, V, c.text_pad, c.text_eos, c.text_unk, unk_penalty, K, cv.data_ptr(),
+                                     ci.data_ptr(), el.data_ptr(), st))
         check(lib.sb_beam_step(Ct.byref(d), st))
         check(lib.sb_step_advance(step.data_ptr(), st))
         if int(fin["active"].item()) == 0:
@@ -699,7 +706,7 @@ def test_search_integer_half_is_bit_exact_on_oracle_logits(tiny):
         trace = {"sentence": sentence}
         uo.generate(fb, None, "spa", hard_max=30, output_units=False, trace=trace)
         prefix = [cfg.text_eos, tiny["toks"][0].lang_index("spa")]
-        decisions, finished = _replay_search_on_logits(eng, trace, prefix, 5, cfg.text_vocab)
+        decisions, finished = _replay_search_on_logits(eng.cfg, trace, prefix, 5, cfg.text_vocab)
         assert len(decisions) == len(trace["beam_idx"])
         for s, (parents, toks) in enumerate(decisions):
             assert parents == trace["beam_idx"][s].tolist(), f"step {s}: parent beams differ"
@@ -722,7 +729,7 @@ def test_search_integer_half_is_bit_exact_on_oracle_logits_at_300_positions(tiny
         assert trace["max_len"] == 300
         if min_len == 298:
             assert len(trace["logits"]) == 300 - len(prefix)  # the search ran to the forced EOS
-        decisions, finished = _replay_search_on_logits(eng, trace, prefix, 5, cfg.text_vocab, min_len=min_len)
+        decisions, finished = _replay_search_on_logits(eng.cfg, trace, prefix, 5, cfg.text_vocab, min_len=min_len)
         assert len(decisions) == len(trace["beam_idx"]) > 200
         for s, (parents, toks) in enumerate(decisions):
             assert parents == trace["beam_idx"][s].tolist(), f"min_len {min_len}, step {s}: parent beams differ"
@@ -798,7 +805,7 @@ def test_full_width_s2st_matches_oracle(base, ops):
     if hyps[0][0][1] == ids:
         assert rel(got.buf.view(1, -1, M), ref["dec_out"]) < 5e-3
     # --- integer half, bit-exact on the oracle's logits at V = 256 102
-    decisions, finished = _replay_search_on_logits(eng, trace, prefix, 5, cfg.text_vocab)
+    decisions, finished = _replay_search_on_logits(eng.cfg, trace, prefix, 5, cfg.text_vocab)
     for s, (parents, toks) in enumerate(decisions):
         assert parents == trace["beam_idx"][s].tolist(), f"step {s}: parent beams differ"
         if s + 1 < len(trace["inputs"]):

@@ -207,13 +207,15 @@ def _tile_stats(lg, V):
     return torch.stack([m, s], -1).transpose(0, 1).contiguous()  # [tile][row][2]
 
 
-def _topk(lg, V, K, pad, eos, unk, pen, bans=None, tiles=False):
+def _topk(lg, V, K, pad, eos, unk, pen, bans=None, tiles=False, stats=None):
+    """`stats`: the tile statistics of `lg` for the tile path (default: _tile_stats)."""
     lib, check = _lib()
     R, ld = lg.shape
     cv = torch.empty((R, K), device=dev)
     ci = torch.empty((R, K), dtype=torch.int32, device=dev)
     el = torch.empty((R,), device=dev)
-    stats = _tile_stats(lg, V) if tiles else None
+    if tiles and stats is None:
+        stats = _tile_stats(lg, V)
     if bans is None:
         if tiles:
             check(lib.sb_logits_topk_tiles(lg.data_ptr(), ld, stats.data_ptr(), R, V, pad, eos, unk, pen, K, cv.data_ptr(), ci.data_ptr(),

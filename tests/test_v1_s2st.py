@@ -173,14 +173,16 @@ def test_t2st_on_v1_still_raises():
 
 
 # ------------------------------------------------------------------------------------------------ GPU
-def with_reachable_eos(sd, cfg, scale=3.0, seed=11):
+def with_reachable_eos(sd, cfg, scale=3.0, seed=11, text=False):
     """The synthetic T2U scores EOS 0, so every search runs to its budget.  An EOS row `scale` times the other rows'
     spread makes some unit searches end early (on the inputs below: 7, 11, 31 and 40 units of 40), so EOS termination
-    and ragged unit lengths reach the vocoder."""
-    e = sd["t2u_model.final_proj.weight"].clone()
+    and ragged unit lengths reach the vocoder.  `text`: the same for the text decoder's tied projection."""
+    proj, embed, eos = (("final_proj.weight", "text_decoder_frontend.embed.weight", cfg.text_eos) if text else
+                        ("t2u_model.final_proj.weight", "t2u_model.decoder_frontend.embed.weight", cfg.unit_eos))
+    e = sd[proj].clone()
     g = torch.Generator().manual_seed(seed)
-    e[cfg.unit_eos] = (torch.randn(cfg.model_dim, generator=g) * scale * 0.25 * cfg.model_dim ** -0.5).half().float()
-    return {**sd, "t2u_model.final_proj.weight": e, "t2u_model.decoder_frontend.embed.weight": e}
+    e[eos] = (torch.randn(cfg.model_dim, generator=g) * scale * 0.25 * cfg.model_dim ** -0.5).half().float()
+    return {**sd, proj: e, embed: e}
 
 
 @pytest.fixture(scope="module")
