@@ -306,6 +306,15 @@ int sb_logits_topk_tiles(const float* logits, int64_t ld, const float* tile_stat
 int sb_ban_step(const int32_t* seqs, int32_t seq_ld, const int32_t* step_ptr, int32_t rows, const int32_t* table, int32_t cap,
                 int32_t width, int32_t* ban_ids, int32_t* ban_n, sb_stream_t stream);
 
+/* N-gram repeat blocking (fairseq2 NGramRepeatBlockProcessor(n)) at one selecting step, in sb_ban_step's output format.
+ * Row r of seqs [rows][seq_ld] holds its hypothesis up to t = *step_ptr (t >= seq_ld reads as seq_ld - 1).  For every start
+ * i with i + n - 1 <= t and seqs[r][i .. i+n-2] == seqs[r][t-n+2 .. t], row r bans seqs[r][i+n-1] (n = 1: every token
+ * seqs[r][0 .. t]); a row of fewer than n tokens bans nothing.  Writes ban_n[r] and the ids to ban_ids[r*cap ..]
+ * (unordered, duplicates possible).  SB_EINVAL before launching for n < 1, cap < max(1, seq_ld - n + 1) (the most starts a
+ * row can have: cap = seq_ld always suffices) or a buffer that is not 4-byte aligned. */
+int sb_ngram_ban_step(const int32_t* seqs, int32_t seq_ld, const int32_t* step_ptr, int32_t rows, int32_t n, int32_t cap,
+                      int32_t* ban_ids, int32_t* ban_n, sb_stream_t stream);
+
 /* sb_logits_topk / sb_logits_topk_tiles with row r's ids ban_ids[r*ban_ld .. + ban_n[r]] banned: a banned id is never a
  * candidate, and eos_lprob is -inf when eos_idx is banned.  The log-sum-exp still runs over the whole row, so every other
  * lprob is the one the unbanned entry returns, bit for bit.  Any number of bans per row: the vocabulary bitmap takes

@@ -86,6 +86,7 @@ PROTOTYPES = {
     "sb_beam_step": [C.POINTER(BeamDesc), c_p],
     "sb_token_timestamps": [c_p, i32, i32, c_p, i32, c_p, c_p, i32, i32, i32, c_p, i64, c_p, i32, c_p],
     "sb_ban_step": [c_p, i32, c_p, i32, c_p, i32, i32, c_p, c_p, c_p],
+    "sb_ngram_ban_step": [c_p, i32, c_p, i32, i32, i32, c_p, c_p, c_p],
     "sb_logits_topk_ban": [c_p, i64, i32, i32, i32, i32, i32, f32, i32, c_p, c_p, c_p, c_p, c_p, i32, c_p],
     "sb_logits_topk_tiles_ban": [c_p, i64, c_p, i32, i32, i32, i32, i32, f32, i32, c_p, c_p, c_p, c_p, c_p, i32, c_p],
     "sb_text_to_chars": [c_p, i32, i32, c_p, c_p, c_p, i32, i32, i32, i32, c_p, c_p, i32, c_p, c_p],

@@ -950,6 +950,34 @@ __global__ void __launch_bounds__(256) ban_step_kernel(const int* __restrict__ s
   if (threadIdx.x == 0) ban_n[r] = s_n;
 }
 
+// N-gram repeat blocking at one selecting step (fairseq2 NGramRepeatBlockProcessor): row r holds seqs[r][0 .. t], t =
+// *step_ptr, prompt included and already in beam order.  Every start i with i + n - 1 <= t whose n-1 tokens
+// seqs[r][i .. i+n-2] equal the row's last n-1 tokens seqs[r][t-n+2 .. t] bans seqs[r][i+n-1], the token that would
+// repeat that n-gram (n = 1: every token of the row).  A row of fewer than n tokens has no start and bans nothing.  One
+// thread per start; the row's last n-1 tokens are the same addresses for every thread.  Output: the sb_ban_step format,
+// at most t - n + 2 <= cap ids per row.
+__global__ void __launch_bounds__(256) ngram_ban_step_kernel(const int* __restrict__ seqs, int seq_ld, const int* __restrict__ step_ptr,
+                                                             int n, int cap, int* __restrict__ ban_ids, int* __restrict__ ban_n) {
+  __shared__ int s_n;
+  pdl_sync();
+  const int r = blockIdx.x;
+  const int t = min(*step_ptr, seq_ld - 1);
+  const int last = t - n + 2;  // first of the row's last n-1 positions
+  const int* row = seqs + (long long)r * seq_ld;
+  if (threadIdx.x == 0) s_n = 0;
+  __syncthreads();
+  for (int i = threadIdx.x; i + n - 1 <= t; i += blockDim.x) {
+    bool hit = true;
+    for (int k = 0; hit && k < n - 1; ++k) hit = row[i + k] == row[last + k];
+    if (hit) {
+      const int slot = atomicAdd(&s_n, 1);
+      if (slot < cap) ban_ids[(long long)r * cap + slot] = row[i + n - 1];
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) ban_n[r] = min(s_n, cap);
+}
+
 // hist[step][...] = h: keeps the final-LayerNorm decoder state of every search step so that the states of the winning
 // hypothesis can be gathered afterwards instead of re-running the decoder teacher-forced (inference/generator.py:294-299)
 __global__ void store_step_kernel(const uint4* __restrict__ h, uint4* __restrict__ hist, const int* __restrict__ step_ptr, long long n16) {
@@ -1256,6 +1284,22 @@ extern "C" int sb_ban_step(const int32_t* seqs, int32_t seq_ld, const int32_t* s
   SB_CUDA_OK(prefer_shared(ban_step_kernel));
   SB_CUDA_OK(launch_k(ban_step_kernel, dim3(rows), dim3(256), 0, (cudaStream_t)stream, (const int*)seqs, (int)seq_ld,
                        (const int*)step_ptr, (const int*)table, (int)cap, (int)width, (int*)ban_ids, (int*)ban_n));
+  count_launch();
+  return SB_OK;
+}
+
+extern "C" int sb_ngram_ban_step(const int32_t* seqs, int32_t seq_ld, const int32_t* step_ptr, int32_t rows, int32_t n,
+                                 int32_t cap, int32_t* ban_ids, int32_t* ban_n, sb_stream_t stream) {
+  using namespace sb;
+  SB_REQUIRE(seqs && step_ptr && ban_ids && ban_n && rows > 0 && seq_ld > 0, SB_EINVAL, "sb_ngram_ban_step: bad args");
+  SB_REQUIRE(n >= 1, SB_EINVAL, "sb_ngram_ban_step: n-gram size %d (>= 1)", n);
+  SB_REQUIRE(cap >= 1 && (int64_t)cap >= (int64_t)seq_ld - n + 1, SB_EINVAL,
+             "sb_ngram_ban_step: cap %d below the %lld starts a row of %d tokens can have", cap, (long long)seq_ld - n + 1, seq_ld);
+  SB_REQUIRE(((uintptr_t)seqs | (uintptr_t)step_ptr | (uintptr_t)ban_ids | (uintptr_t)ban_n) % 4 == 0, SB_EINVAL,
+             "sb_ngram_ban_step: buffers must be 4-byte aligned");
+  SB_CUDA_OK(prefer_shared(ngram_ban_step_kernel));
+  SB_CUDA_OK(launch_k(ngram_ban_step_kernel, dim3(rows), dim3(256), 0, (cudaStream_t)stream, (const int*)seqs, (int)seq_ld,
+                       (const int*)step_ptr, (int)n, (int)cap, (int*)ban_ids, (int*)ban_n));
   count_launch();
   return SB_OK;
 }

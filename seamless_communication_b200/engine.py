@@ -392,12 +392,13 @@ class UnitYEngine:
         check(lib.sb_store_step(h.buf.data_ptr(), st["hist"].data_ptr(), st["step"].data_ptr(), R * M * 2, stream), "sb_store_step")
         ops.gemm(h, w["text_embed"], c.text_vocab, None, out=st["logits"], out_f32=True, tile_stats=st["tile_stats"])
 
-    def _topk(self, st, eos_idx, unk_penalty, ban=False):
+    def _topk(self, st, eos_idx, unk_penalty, bans=None):
         """log-softmax statistics + top-K candidates of every row (st["logits"] / st["tile_stats"] of the last projection).
-        `ban`: the ids sb_ban_step wrote to st["ban_ids"] are not candidates."""
+        `bans`: a ban-list buffer of the state (st["ban"] or st["ngram"]); the ids written to its `ids` / `n` are not
+        candidates."""
         lib, c = _lib.load(), self.cfg
-        if ban:
-            b = st["ban"]
+        if bans is not None:
+            b = bans
             if st["tile_stats"] is not None:
                 check(lib.sb_logits_topk_tiles_ban(st["logits"].buf.data_ptr(), st["logits"].buf.stride(0), st["tile_stats"].data_ptr(),
                                                    st["R"], c.text_vocab, c.text_pad, eos_idx, c.text_unk, unk_penalty, st["K"],
@@ -419,14 +420,20 @@ class UnitYEngine:
                                      eos_idx, c.text_unk, unk_penalty, st["K"], st["cand_val"].data_ptr(),
                                      st["cand_idx"].data_ptr(), st["eos_lprob"].data_ptr(), ops._stream()), "sb_logits_topk")
 
-    def _decoder_step_select(self, st, ban=False):
+    def _decoder_step_select(self, st, ban=False, ngram=0):
+        """`ban`: banned sequences (sb_ban_step on st["ban"]); `ngram` > 0: n-gram repeat blocking of that size
+        (sb_ngram_ban_step on st["ngram"]).  Either feeds the ban-aware top-K."""
         lib = _lib.load()
         stream = ops._stream()
+        bans = None
         if ban:
-            b = st["ban"]
+            b = bans = st["ban"]
             check(lib.sb_ban_step(st["seqs"].data_ptr(), st["ML"], st["step"].data_ptr(), st["R"], b["table"].data_ptr(), b["cap"],
                                   b["width"], b["ids"].data_ptr(), b["n"].data_ptr(), stream), "sb_ban_step")
-        self._topk(st, self.cfg.text_eos, st["unk_penalty"], ban=ban)
+        elif ngram:
+            bans = st["ngram"]
+            ops.ngram_ban_step(st["seqs"], st["step"], ngram, bans["ids"], bans["n"])
+        self._topk(st, self.cfg.text_eos, st["unk_penalty"], bans=bans)
         check(lib.sb_beam_step(C.byref(st["beam_desc"]), stream), "sb_beam_step")
         check(lib.sb_step_advance(st["step"].data_ptr(), stream), "sb_step_advance")
 
@@ -511,10 +518,11 @@ class UnitYEngine:
         d.fin_anc, d.len_budget = fin["anc"].data_ptr(), st["budget"].data_ptr()
         d.fin_scores = fin["scores"].data_ptr()
         st["beam_desc"] = d
-        st["g_fwd"] = st["g_sel"] = st["g_sel_ban"] = st["g_fwd_attn"] = None
-        st["n_fwd"] = st["n_sel"] = st["n_sel_ban"] = st["n_fwd_attn"] = 0
+        st["g_fwd"] = st["g_sel"] = st["g_sel_ban"] = st["g_fwd_attn"] = st["g_sel_ngram"] = None
+        st["n_fwd"] = st["n_sel"] = st["n_sel_ban"] = st["n_fwd_attn"] = st["n_sel_ngram"] = 0
         st["attn_hist"], st["attn_on"] = None, False  # [ML][R][S_enc] fp32, allocated by the first recording search
         st["ban"], st["ban_on"] = None, False
+        st["ngram"], st["ngram_on"] = None, 0  # ban lists of n-gram blocking, allocated by the first blocking search
         self._graphs[key] = st
         self._evict_search_states(keep=key)
         return st
@@ -582,17 +590,25 @@ class UnitYEngine:
     def _capture_ban(self, st):
         """Capture the select half with banned sequences (sb_ban_step, ban-aware top-K, sb_beam_step, sb_step_advance) on the
         state's ban table; searches without bans keep replaying g_sel."""
+        self._capture_select(st, "g_sel_ban", "n_sel_ban", ban=True)
+
+    def _capture_ngram(self, st):
+        """Capture the select half with n-gram repeat blocking of size st["ngram"]["size"] (sb_ngram_ban_step, ban-aware
+        top-K, sb_beam_step, sb_step_advance) on the state's ban lists; searches without blocking keep replaying g_sel."""
+        self._capture_select(st, "g_sel_ngram", "n_sel_ngram", ngram=st["ngram"]["size"])
+
+    def _capture_select(self, st, graph, count, **kw):
         with _CAPTURE_LOCK:
             s = torch.cuda.Stream()
             s.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(s):
-                self._decoder_step_select(st, ban=True)
+                self._decoder_step_select(st, **kw)
             torch.cuda.current_stream().wait_stream(s)
             n0 = ops.launch_count()
-            st["g_sel_ban"] = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(st["g_sel_ban"], stream=_capture_stream(), capture_error_mode="thread_local"):
-                self._decoder_step_select(st, ban=True)
-            st["n_sel_ban"] = ops.launch_count() - n0
+            st[graph] = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(st[graph], stream=_capture_stream(), capture_error_mode="thread_local"):
+                self._decoder_step_select(st, **kw)
+            st[count] = ops.launch_count() - n0
 
     def _capture_attn(self, st):
         """Capture the forward half with the cross-attention weights recorded (sb_decode_cross_attn_weights after the last
@@ -633,6 +649,20 @@ class UnitYEngine:
         b["table"].copy_(host, non_blocking=True)
         b["host"] = host  # the pinned source stays alive until the copy has run
 
+    def _set_ngram(self, st, n):
+        """N-gram blocking of size `n` on this state: ban lists of ML ids per row (a row at step t has at most t-n+2
+        starts, t <= ML-1), allocated once per state.  The captured graph has `n` baked in and is recaptured when it
+        changes."""
+        b = st["ngram"]
+        if b is None:
+            dev = self.device
+            b = st["ngram"] = dict(cap=st["ML"], size=0, ids=torch.zeros((st["R"], st["ML"]), dtype=I32, device=dev),
+                                   n=torch.zeros(st["R"], dtype=I32, device=dev))
+            with self._state_lock:  # the cache budget now counts the lists too
+                self._evict_search_states(keep=st["key"])
+        if b["size"] != n:
+            b["size"], st["g_sel_ngram"] = n, None
+
     def _search_reset(self, st, prefix):
         fin, P = st["fin"], st["P"]
         st["seqs"].zero_()
@@ -644,7 +674,7 @@ class UnitYEngine:
         st["step"].zero_()
 
     def _search_prepare(self, st, enc: Seq, enc_lens, prefix, len_penalty, unk_penalty, min_seq_len, use_graph, max_len,
-                        banned=None, record=False):
+                        banned=None, record=False, ngram=None):
         """(Re)initialise one cached search state in place for the sentences of `enc` and a length budget `max_len`
         (<= the state's allocated length); capture its graphs if needed."""
         c, M = self.cfg, self.M
@@ -654,9 +684,10 @@ class UnitYEngine:
         if st.get("opts_cap") != (min_seq_len, float(len_penalty)) or st.get("unk_cap") != float(unk_penalty):
             d.min_len, d.len_penalty = min_seq_len, len_penalty
             st["opts_cap"] = (min_seq_len, float(len_penalty))  # compared as Python values: c_float rounds 0.9 and would recapture every call
-            st["g_fwd"] = st["g_sel"] = st["g_sel_ban"] = None  # scalar options are baked into the captured select graphs
+            st["g_fwd"] = st["g_sel"] = st["g_sel_ban"] = st["g_sel_ngram"] = None  # scalar options are baked into the captured select graphs
             st["unk_cap"] = float(unk_penalty)
         st["ban_on"] = bool(banned)
+        st["ngram_on"] = ngram or 0
         st["attn_on"] = record
         if record and st["attn_hist"] is None:
             st["attn_hist"] = torch.zeros((st["ML"], st["R"], st["S_enc"]), dtype=torch.float32, device=self.device)
@@ -664,6 +695,8 @@ class UnitYEngine:
                 self._evict_search_states(keep=st["key"])
         if banned:
             self._set_bans(st, banned)
+        if ngram:
+            self._set_ngram(st, ngram)
         if enc_lens is not None:
             st["enc_lens"].copy_(enc_lens)
         for i in range(c.dec_layers):
@@ -675,23 +708,26 @@ class UnitYEngine:
         if use_graph and banned and st["g_sel_ban"] is None:
             self._capture_ban(st)
             self._search_reset(st, prefix)
+        if use_graph and ngram and st["g_sel_ngram"] is None:
+            self._capture_ngram(st)
+            self._search_reset(st, prefix)
         if use_graph and record and st["g_fwd_attn"] is None:
             self._capture_attn(st)
             self._search_reset(st, prefix)
 
     def _search_step(self, st, use_graph, select=True):
-        ban, rec = st["ban_on"], st["attn_on"]
+        ban, ngram, rec = st["ban_on"], st["ngram_on"], st["attn_on"]
         if use_graph:
+            sel = "_ban" if ban else "_ngram" if ngram else ""
             st["g_fwd_attn" if rec else "g_fwd"].replay()
             if select:
-                st["g_sel_ban" if ban else "g_sel"].replay()
+                st["g_sel" + sel].replay()
             with self._count_lock:
-                self.graph_kernels += (st["n_fwd_attn"] if rec else st["n_fwd"]) + \
-                    ((st["n_sel_ban"] if ban else st["n_sel"]) if select else 0)
+                self.graph_kernels += (st["n_fwd_attn"] if rec else st["n_fwd"]) + (st["n_sel" + sel] if select else 0)
         else:
             self._decoder_step_forward(st, record=rec)
             if select:
-                self._decoder_step_select(st, ban=ban)
+                self._decoder_step_select(st, ban=ban, ngram=ngram)
 
     def _search_bootstrap_step(self, st, prefix, i, use_graph):
         """fairseq2.cpp:1162-1247: feed prefix[i], score prefix[i+1] (the top-K kernel reports the lprob of its
@@ -720,7 +756,7 @@ class UnitYEngine:
     @torch.inference_mode()
     def beam_search(self, enc: Seq, enc_lens, prefix: List[int], beam=5, soft_max=(1, 200), hard_max=1024,
                     len_penalty=1.0, unk_penalty=0.0, min_seq_len=1, use_graph=True, cross_kv=None, state_len=None,
-                    banned=None, record_attention=False):
+                    banned=None, record_attention=False, ngram=None):
         """Device-resident beam search.  Returns per sentence the finished hypotheses [(score, ids)], best first
         (semantics: fairseq2.cpp:1371-1608; see decode.cu).  `cross_kv` is ignored (kept for API stability): the
         static cross-attention K/V of the cached search state are recomputed from `enc`.
@@ -730,7 +766,16 @@ class UnitYEngine:
         `banned`: token-id sequences of fairseq2's BannedSequenceProcessor, applied at every selecting step (not in the
         prefix bootstrap): a row whose last n-1 tokens equal a sequence's first n-1 cannot take its last token.
         `record_attention`: every step also keeps the last decoder layer's head-summed cross-attention weights, for
-        `token_timestamps` (one more kernel per step, on a third captured graph of the state)."""
+        `token_timestamps` (one more kernel per step, on a third captured graph of the state).
+        `ngram`: the n-gram size of fairseq2's NGramRepeatBlockProcessor, applied where `banned` is: at every selecting
+        step a row cannot take a token that would repeat one of its n-grams (the prompt's included).  Not combined with
+        `banned`."""
+        if ngram is not None:
+            if isinstance(ngram, bool) or int(ngram) != ngram or ngram < 1:
+                raise ValueError(f"the n-gram size must be an integer >= 1, got {ngram!r}")
+            if banned:
+                raise NotImplementedError("banned sequences and n-gram blocking cannot be combined in one search")
+            ngram = int(ngram)
         if banned is not None:
             banned = [[int(t) for t in (x.tolist() if isinstance(x, torch.Tensor) else x)] for x in banned]
             V = self.cfg.text_vocab
@@ -751,7 +796,7 @@ class UnitYEngine:
         ML_state = ML if state_len is None else max(ML, int(state_len))
         st = self._search_state(B, S_enc, ML_state, beam, P, enc_lens is not None, use_graph)
         self._search_prepare(st, enc, enc_lens, prefix, len_penalty, unk_penalty, min_seq_len, use_graph, ML, banned,
-                             bool(record_attention))
+                             bool(record_attention), ngram)
         n_steps = ML - 1 - (P - 1)
         for i in range(P - 1):
             self._search_bootstrap_step(st, prefix, i, use_graph)

@@ -58,6 +58,28 @@ class BannedSequenceProcessor:
         self.banned_seqs: List[List[int]] = seqs
 
 
+class NGramRepeatBlockProcessor:
+    """fairseq2's `NGramRepeatBlockProcessor`, the step processor of the reference CLI's `--text_generation_ngram_blocking`
+    / `--unit_generation_ngram_blocking` (`--no_repeat_ngram_size`): at every selecting step of the search, a hypothesis
+    cannot take a token that would complete an n-gram it already holds (its prompt included; n = 1: any token it holds).
+    The search applies it on the device (engine.beam_search `ngram`, decode.cu sb_ngram_ban_step); this object only holds
+    and checks the size."""
+
+    def __init__(self, ngram_size: int) -> None:
+        if ngram_size < 1:
+            raise ValueError("`ngram_size` must be greater than 0.")
+        self.ngram_size = int(ngram_size)
+
+
+def _search_processor(p) -> dict:
+    """The beam_search keywords of a step processor the device search runs."""
+    if isinstance(p, BannedSequenceProcessor):
+        return dict(banned=p.banned_seqs)
+    if isinstance(p, NGramRepeatBlockProcessor):
+        return dict(ngram=p.ngram_size)
+    return {}
+
+
 @dataclass
 class SequenceGeneratorOptions:
     """generator.py:59-84 (same fields and defaults)."""
@@ -90,8 +112,9 @@ class UnitYGenerator:
         if model.text_decoder is None:
             raise ValueError("`UnitYGenerator` requires a text decoder, but the current UnitY model does not have one.")
         p = self.text_opts.step_processor
-        if p is not None and not isinstance(p, BannedSequenceProcessor):
-            raise NotImplementedError("the text search supports BannedSequenceProcessor as its only step processor")
+        if p is not None and not isinstance(p, (BannedSequenceProcessor, NGramRepeatBlockProcessor)):
+            raise NotImplementedError("the text search supports BannedSequenceProcessor and NGramRepeatBlockProcessor as "
+                                      "its step processors")
         self.text_tokenizer = text_tokenizer
         enc = text_tokenizer.create_encoder(task="translation", lang=target_lang, mode="target")
         self.prefix = enc.prefix_indices.tolist()  # [</s>, __lang__]
@@ -104,8 +127,10 @@ class UnitYGenerator:
                 raise ValueError("`model` does not have a T2U sub-model when `unit_tokenizer` is not None.")
             self.unit_decoder = unit_tokenizer.create_decoder()
             self.unit_prefix_indices = unit_tokenizer.create_encoder(lang=target_lang).prefix_indices
-            if isinstance(model.t2u_model, UnitYT2UModel) and self.unit_opts.step_processor is not None:
-                raise NotImplementedError("step processors are not supported on the unit search")
+            # the NAR T2U has no search: the reference does not read the unit options there, and neither does this
+            up = self.unit_opts.step_processor
+            if isinstance(model.t2u_model, UnitYT2UModel) and up is not None and not isinstance(up, NGramRepeatBlockProcessor):
+                raise NotImplementedError("the unit search supports NGramRepeatBlockProcessor as its only step processor")
 
     @torch.inference_mode()
     def __call__(self, source_seqs: Tensor, source_padding_mask: Optional[PaddingMask], input_modality: str = "speech",
@@ -124,10 +149,9 @@ class UnitYGenerator:
         enc = Seq(B, S, M, buf=enc_out.view(B * S, M))
         enc_lens = None if enc_mask is None else enc_mask.seq_lens.to(device=enc_out.device, dtype=I32)
         o = self.text_opts
-        banned = o.step_processor.banned_seqs if o.step_processor is not None else None
         hyps = eng.beam_search(enc, enc_lens, self.prefix, beam=o.beam_size, soft_max=o.soft_max_seq_len,
                                hard_max=o.hard_max_seq_len, len_penalty=o.len_penalty, unk_penalty=o.unk_penalty,
-                               banned=banned)
+                               **_search_processor(o.step_processor))
         for h in hyps:
             if not h:
                 raise RuntimeError("The sequence generator returned no hypothesis at index 0. Please file a bug report.")
@@ -167,7 +191,7 @@ class UnitYGenerator:
         o = self.unit_opts
         hyps = t2u.beam_search(t2u_enc, text_lens, self.unit_prefix_indices.tolist(), beam=o.beam_size,
                                soft_max=o.soft_max_seq_len, hard_max=o.hard_max_seq_len, len_penalty=o.len_penalty,
-                               unk_penalty=o.unk_penalty)
+                               unk_penalty=o.unk_penalty, **_search_processor(o.step_processor))
         for h in hyps:
             if not h:
                 raise RuntimeError("The sequence generator returned no hypothesis at index 0. Please file a bug report.")

@@ -102,14 +102,15 @@ class UnitYT2UModel:
         return _project(self.unit_engine, decoder_output, self.target_vocab_info)
 
     def beam_search(self, enc: Seq, enc_lens: Optional[Tensor], prefix: List[int], beam=5, soft_max=(25, 50),
-                    hard_max=1024, len_penalty=1.0, unk_penalty=0.0, bucket: bool = True):
+                    hard_max=1024, len_penalty=1.0, unk_penalty=0.0, bucket: bool = True, ngram: Optional[int] = None):
         """Unit beam search of BeamSearchSeq2SeqGenerator(echo_prompt=True) over the T2U encoder output `enc` (B, S, M)
         with per-row lengths `enc_lens` (int32 on the device; None: every row has S).  The length budget
         min(hard_max, a*S + b) uses the unpadded S, as the reference does.  With `bucket` (the results are the same):
           * the rows are padded to a multiple of S_ENC_BUCKET, masked through the lengths;
           * the search state is allocated for min(hard_max, unit_max_seq_len) positions (at least the budget), and the
             budget is applied on the device,
-        so every text length of one bucket searches on one cached state with the same captured graphs."""
+        so every text length of one bucket searches on one cached state with the same captured graphs.
+        `ngram`: n-gram repeat blocking of that size (NGramRepeatBlockProcessor on the unit options; engine.beam_search)."""
         a, b = soft_max
         max_len = hard_max if a <= 0 else min(hard_max, int(a * enc.T) + b)
         state_len = None
@@ -126,7 +127,7 @@ class UnitYT2UModel:
                 # (decode_full reuses that search's cross-attention K/V), so the address must not go to another tensor
                 self._tls.padded_enc = buf
         return self.unit_engine.beam_search(enc, enc_lens, prefix, beam=beam, soft_max=(0, 0), hard_max=max_len,
-                                            len_penalty=len_penalty, unk_penalty=unk_penalty, state_len=state_len)
+                                            len_penalty=len_penalty, unk_penalty=unk_penalty, state_len=state_len, ngram=ngram)
 
 
 class UnitYNART2UModel:

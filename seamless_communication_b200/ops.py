@@ -385,6 +385,17 @@ def decode_cross_attn_weights(q_partials: torch.Tensor, splits: int, slice_rows:
                                                    heads, _stream()), "sb_decode_cross_attn_weights")
 
 
+def ngram_ban_step(seqs: torch.Tensor, step: torch.Tensor, n: int, ban_ids: torch.Tensor, ban_n: torch.Tensor) -> None:
+    """N-gram repeat blocking at one selecting step (sb_ngram_ban_step): row r of seqs (rows, seq_ld) int32, read up to the
+    device step index step[0], bans the token after every earlier occurrence of its last n-1 tokens.  Writes the ids to
+    ban_ids (rows, cap) int32, cap >= seq_ld - n + 1, and their count to ban_n (rows,) int32 - the lists the `_ban` top-K
+    entry points read (ban_ld = cap)."""
+    if not (seqs.is_contiguous() and ban_ids.is_contiguous()):
+        raise ValueError("ngram_ban_step needs contiguous seqs and ban_ids")
+    check(_lib.load().sb_ngram_ban_step(seqs.data_ptr(), seqs.shape[1], step.data_ptr(), seqs.shape[0], int(n), ban_ids.shape[1],
+                                        ban_ids.data_ptr(), ban_n.data_ptr(), _stream()), "sb_ngram_ban_step")
+
+
 def token_timestamps(hist: torch.Tensor, slots: torch.Tensor, n_tok: torch.Tensor, enc_lens: Optional[torch.Tensor],
                      prefix_len: int, width: int) -> torch.Tensor:
     """Start bins (B, max(n_tok)) int32 of each row's tokens from the attention history hist (max_len, rows, s_enc) fp32
