@@ -101,6 +101,20 @@ int sb_gemm_splitk(const sb_gemm_t* g, int32_t splits, float* partials, int64_t 
  * steps; tests/test_decode_gemm.py checks it), so the decoder step's outputs do not depend on the path. */
 int sb_gemm_decode_supported(const sb_gemm_t* g, int32_t splits);
 int sb_gemm_decode(const sb_gemm_t* g, int32_t splits, float* partials, int64_t slice_rows, sb_stream_t stream);
+/* FP8 decoder weights (weight-only E4M3, DESIGN.md section 16): the same products with `w` pointing to [n][c_in] e4m3fn
+ * bytes and w_scale to one fp32 scale per output feature (a power of two).  The weight tile is converted to fp16 in
+ * shared memory and runs the same MMAs in the same order, and the epilogue starts from acc * w_scale[feature]: the
+ * results equal sb_gemm_decode's on the fp16 weights q * scale, bit for bit.  Any row count: more than 256 rows run in
+ * chunks of 256.  SB_EINVAL for a NULL or misaligned w_scale, misaligned operands, or a shape sb_gemm_decode refuses
+ * at <= 256 rows. */
+int sb_gemm_decode_e4m3(const sb_gemm_t* g, const float* w_scale, int32_t splits, float* partials, int64_t slice_rows,
+                        sb_stream_t stream);
+/* The tied vocabulary projection on e4m3 weights: out[r][v] = (h[r] . (q[v] * w_scale[v]) + bias[v]) * alpha * gamma
+ * (fp32, out_f32 = 1) with, when tile_stats is set, its per-(128-column tile, row) log-softmax statistics - what
+ * sb_gemm with tile_stats writes for the fp16 weights q * scale, bit for bit.  Any row count (chunks of 256).
+ * SB_EINVAL for a NULL or misaligned w_scale, misaligned operands, act != none, a prefetch range, or a shape the
+ * fp16 projection refuses. */
+int sb_vocab_proj_e4m3(const sb_gemm_t* g, const float* w_scale, sb_stream_t stream);
 /* consumer of the partials: x += bias + sum_z partial[z] (x fp16 [rows][dim], updated in place) and h = LayerNorm(x).
  * Fuses the reduction into the LayerNorm that follows every residual GEMM of a pre-LN decoder layer
  * (StandardTransformerDecoderLayer, fairseq2.cpp:979-1060). */

@@ -59,6 +59,8 @@ PROTOTYPES = {
     "sb_gemm_splitk": [C.POINTER(GemmDesc), i32, c_p, i64, c_p],
     "sb_gemm_decode_supported": [c_p, i32],
     "sb_gemm_decode": [c_p, i32, c_p, i64, c_p],
+    "sb_gemm_decode_e4m3": [c_p, c_p, i32, c_p, i64, c_p],
+    "sb_vocab_proj_e4m3": [C.POINTER(GemmDesc), c_p, c_p],
     "sb_splitk_reduce_ln": [c_p, i32, i32, i64, i32, c_p, c_p, c_p, c_p, c_p, c_p],
     "sb_fbank": [c_p, i64, c_p, i32, c_p, i32, c_p, c_p, i32, c_p],
     "sb_layernorm": [c_p, c_p, c_p, c_p, c_p, c_p, i32, i32, i32, i32, i32, i32, i32, c_p, i32, c_p],

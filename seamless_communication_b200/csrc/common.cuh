@@ -66,7 +66,8 @@ __device__ __forceinline__ void pdl_sync() { pdl_wait(); pdl_trigger(); }
 
 bool pdl_enabled();
 int sm_count();  // SMs of the current device (cached per device)
-// 2D fp16 (esize 2) / fp32 (esize 4) tensor map: inner = channels, box 128 B x box_rows, 128B swizzle, OOB -> 0 (gemm_tcgen05.cu)
+// 2D fp16 (esize 2) / fp32 (esize 4) tensor map: inner = channels, box 128 B x box_rows, 128B swizzle, OOB -> 0 (gemm_tcgen05.cu);
+// esize 1 (e4m3 bytes): box 64 B x box_rows, no swizzle
 int make_tmap(CUtensorMap* tm, const void* base, uint64_t inner, uint64_t rows, uint64_t ld_elems, uint32_t box_rows,
               int esize = 2);
 // sb_gemm with tile_stats at <= 256 rows on the weight-stationary projection kernel (decode_gemm.cu).  Returns false,

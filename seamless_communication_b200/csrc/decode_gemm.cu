@@ -85,10 +85,24 @@ struct DgArgs {
 
 __device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }  // warps 0-7
 
-// Shared memory: `stages` ring stages, `extra` bytes (the projection's staging buffer), the full / empty barriers.
-template <int NT>
+// the two e4m3 bytes in the low half of v -> fp16x2, low byte to the low half (exact: every e4m3 value is an fp16 value)
+__device__ __forceinline__ uint32_t e4m3x2_to_f16x2(uint32_t v) {
+  uint32_t r;
+  asm("{.reg .b16 t; cvt.u16.u32 t, %1; cvt.rn.f16x2.e4m3x2 %0, t;}" : "=r"(r) : "r"(v));
+  return r;
+}
+
+// Shared memory: `stages` ring stages, the fp16 copies of the e4m3 weight tile (F8), `extra` bytes (the projection's
+// staging buffer), the full / empty barriers.
+// F8: the ring's weight tile is [128 features][64] e4m3 bytes (unswizzled 64-byte rows: half the bytes of the fp16
+// tile).  Each consumer warpgroup converts its 64 rows into fp16 in the 128B-swizzled layout TMA writes for an fp16
+// tile, in a buffer of its own alternating between k-blocks (the k-block before the last may still be in flight), and
+// the wgmma reads that buffer through the same descriptors: the same m64 x k16 steps on the same values q.
+template <int NT, bool F8 = false>
 struct Ring {
-  static constexpr int STAGE_BYTES = DG_W_BYTES + NT * DG_BK * 2;
+  static constexpr int W_BYTES = F8 ? DG_TM * DG_BK : DG_W_BYTES;  // weight tile bytes per stage
+  static constexpr int STAGE_BYTES = W_BYTES + NT * DG_BK * 2;
+  static constexpr int CONV_BYTES = F8 ? 2 * DG_W_BYTES : 0;       // F8: two fp16 weight tiles
   static constexpr int GROUP_BYTES = NT * 128;           // projection: [NT rows][32 fp32], one TMA store box
   static constexpr int STAGING_BYTES = 2 * GROUP_BYTES;  // projection: one 64-feature half of a tile
   static_assert(NT % 16 == 0 && NT <= 256, "wgmma N");
@@ -100,7 +114,7 @@ struct Ring {
 
   __device__ Ring(uint8_t* raw, int n, int extra)
       : smem((uint8_t*)(((uintptr_t)raw + 1023) & ~(uintptr_t)1023)),
-        full((uint64_t*)(smem + (size_t)n * STAGE_BYTES + extra)),
+        full((uint64_t*)(smem + (size_t)n * STAGE_BYTES + CONV_BYTES + extra)),
         empty(full + DG_MAX_STAGES),
         stages(n) {}
 
@@ -128,12 +142,39 @@ struct Ring {
         mbar_expect_tx(&full[s], STAGE_BYTES);
         tma_load_2d(st, &tmW, &full[s], kb * DG_BK, tile * DG_TM);
         if (!waited) pdl_wait();
-        tma_load_2d(st + DG_W_BYTES, &tmX, &full[s], kb * DG_BK, 0);
+        tma_load_2d(st + W_BYTES, &tmX, &full[s], kb * DG_BK, 0);
       }
       waited = true;
       __syncwarp();
       advance();
     }
+  }
+
+  // F8 consumer warpgroup: its 64 rows of the stage's e4m3 tile -> fp16 buffer `buf`; returns the buffer's address.
+  // Warp w converts rows 16w .. 16w+15, the A rows of its own part of the m64 MMA, in 16-byte chunks (one row = 4
+  // chunks = 8 chunks of the fp16 row, stored at chunk j ^ (row & 7)).  That k-block's MMAs were the last to read the
+  // buffer two k-blocks ago and have completed (wg_wait<1>).
+  __device__ __forceinline__ uint32_t to_f16(const uint8_t* stage, int buf) {
+    const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+    const uint8_t* src = stage + wg * 64 * DG_BK;
+    uint8_t* dst = smem + (size_t)stages * STAGE_BYTES + buf * DG_W_BYTES + wg * 64 * 128;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int c = (t >> 5) * 64 + (t & 31) + 32 * i;  // chunk: row c / 4, bytes 16 (c % 4) ..
+      const int r = c >> 2, j = (c & 3) * 2;
+      const uint4 v = *reinterpret_cast<const uint4*>(src + c * 16);
+      uint4 lo, hi;
+      lo.x = e4m3x2_to_f16x2(v.x); lo.y = e4m3x2_to_f16x2(v.x >> 16);
+      lo.z = e4m3x2_to_f16x2(v.y); lo.w = e4m3x2_to_f16x2(v.y >> 16);
+      hi.x = e4m3x2_to_f16x2(v.z); hi.y = e4m3x2_to_f16x2(v.z >> 16);
+      hi.z = e4m3x2_to_f16x2(v.w); hi.w = e4m3x2_to_f16x2(v.w >> 16);
+      *reinterpret_cast<uint4*>(dst + r * 128 + ((j ^ (r & 7)) << 4)) = lo;
+      *reinterpret_cast<uint4*>(dst + r * 128 + (((j + 1) ^ (r & 7)) << 4)) = hi;
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> wgmma (async proxy) reads
+    if (wg == 0) asm volatile("bar.sync 2, 128;" ::: "memory");      // the warpgroup's four warps
+    else asm volatile("bar.sync 3, 128;" ::: "memory");
+    return smem_u32(dst - wg * 64 * 128);
   }
 
   // Consumer warpgroups: acc = D[feature][row] = W[64 features of warpgroup wg] . X[NT rows]^T over k-blocks [kb0, kb1).
@@ -146,7 +187,9 @@ struct Ring {
     for (int kb = kb0; kb < kb1; ++kb) {
       mbar_wait(&full[s], ph);
       const uint32_t sa = smem_u32(smem + (size_t)s * STAGE_BYTES);
-      const uint64_t da = make_smem_desc(sa + wg * 64 * 128), db = make_smem_desc(sa + DG_W_BYTES);
+      uint32_t sw = sa;
+      if constexpr (F8) sw = to_f16(smem + (size_t)s * STAGE_BYTES, (kb - kb0) & 1);
+      const uint64_t da = make_smem_desc(sw + wg * 64 * 128), db = make_smem_desc(sa + W_BYTES);
       wg_fence();
 #pragma unroll
       for (int k = 0; k < DG_BK / 16; ++k) Wgmma<NT>::mma(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2));
@@ -163,11 +206,13 @@ struct Ring {
   }
 };
 
-template <int NT>
-__global__ void __launch_bounds__(DG_THREADS, 1)
-decode_gemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const DgArgs g) {
+// F8: tmW maps e4m3 weights and w_scale holds one fp32 scale per feature; the epilogue starts from acc * w_scale[feature]
+// (a power of two, so that product is exactly the accumulator of the fp16 weights q * scale)
+template <int NT, bool F8>
+__device__ __forceinline__ void decode_gemm_body(const CUtensorMap& tmW, const CUtensorMap& tmX, const DgArgs g,
+                                                 const float* w_scale) {
   extern __shared__ uint8_t smem_raw[];
-  Ring<NT> ring(smem_raw, g.stages, 0);
+  Ring<NT, F8> ring(smem_raw, g.stages, 0);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int u = blockIdx.x;
   const int tile = u / g.splits, split = u - tile * g.splits;
@@ -199,12 +244,17 @@ decode_gemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
   const int wg = warp >> 2;
   float* stage = reinterpret_cast<float*>(ring.smem);
   const int fl = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  float sc[2] = {1.f, 1.f};
+  if constexpr (F8)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) sc[h] = tile * DG_TM + fl + 8 * h < g.n_out ? w_scale[tile * DG_TM + fl + 8 * h] : 0.f;
 #pragma unroll
   for (int j = 0; j < NT / 8; ++j)
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
-      for (int e = 0; e < 2; ++e) stage[(j * 8 + (lane & 3) * 2 + e) * DG_SP + fl + 8 * h] = acc[j * 4 + 2 * h + e];
+      for (int e = 0; e < 2; ++e)
+        stage[(j * 8 + (lane & 3) * 2 + e) * DG_SP + fl + 8 * h] = F8 ? acc[j * 4 + 2 * h + e] * sc[h] : acc[j * 4 + 2 * h + e];
   consumer_bar();
   pdl_sync();
   const int f_tile = tile * DG_TM;
@@ -258,12 +308,26 @@ decode_gemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
 
 template <int NT>
 __global__ void __launch_bounds__(DG_THREADS, 1)
-vocab_proj_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX,
-                  const __grid_constant__ CUtensorMap tmO, const DgArgs g) {
-  using R = Ring<NT>;
+decode_gemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const DgArgs g) {
+  decode_gemm_body<NT, false>(tmW, tmX, g, nullptr);
+}
+
+template <int NT>
+__global__ void __launch_bounds__(DG_THREADS, 1)
+decode_gemm_e4m3_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const DgArgs g,
+                        const float* w_scale) {
+  decode_gemm_body<NT, true>(tmW, tmX, g, w_scale);
+}
+
+// F8 as in decode_gemm_body: logits = (acc * w_scale[feature] + bias) * post_scale.  stats_ld: row stride of tile_stats
+// (the e4m3 entry runs more than 256 rows in chunks that write one statistics array)
+template <int NT, bool F8>
+__device__ __forceinline__ void vocab_proj_body(const CUtensorMap& tmW, const CUtensorMap& tmX, const CUtensorMap& tmO,
+                                                const DgArgs g, const float* w_scale, long long stats_ld) {
+  using R = Ring<NT, F8>;
   extern __shared__ uint8_t smem_raw[];
   R ring(smem_raw, g.stages, R::STAGING_BYTES);
-  uint8_t* staging = ring.smem + (size_t)g.stages * R::STAGE_BYTES;
+  uint8_t* staging = ring.smem + (size_t)g.stages * R::STAGE_BYTES + R::CONV_BYTES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) ring.init(&tmW, &tmX, &tmO);
   __syncthreads();
@@ -301,6 +365,8 @@ vocab_proj_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
           const int fl = (warp & 3) * 16 + (lane >> 2) + 8 * h;  // feature inside the half
           const int f = fq + fl;
           const float b = (g.bias != nullptr && f < g.n_out) ? g.bias[f] : 0.f;
+          float sc = 1.f;
+          if constexpr (F8) sc = f < g.n_out ? w_scale[f] : 0.f;
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             // row r = 8j + r0: the swizzle (r & 7 = r0) does not depend on j, so j only adds an immediate 1 KB offset
@@ -308,7 +374,8 @@ vocab_proj_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
             float* p = reinterpret_cast<float*>(staging + (fl >> 5) * R::GROUP_BYTES + r0 * 128 + ((((fl & 31) >> 2) ^ r0) << 4) +
                                                 (fl & 3) * 4);
 #pragma unroll
-            for (int j = 0; j < NT / 8; ++j) p[j * 256] = (acc[j * 4 + 2 * h + e] + b) * g.post_scale;
+            for (int j = 0; j < NT / 8; ++j)
+              p[j * 256] = ((F8 ? acc[j * 4 + 2 * h + e] * sc : acc[j * 4 + 2 * h + e]) + b) * g.post_scale;
           }
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -343,11 +410,25 @@ vocab_proj_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant
             st_m = nm;
           }
         }
-        if (q == 1) g.tile_stats[(long long)tile * g.rows + row] = make_float2(st_m, st_s);
+        if (q == 1) g.tile_stats[(long long)tile * stats_ld + row] = make_float2(st_m, st_s);
       }
     }
   }
   if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+}
+
+template <int NT>
+__global__ void __launch_bounds__(DG_THREADS, 1)
+vocab_proj_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX,
+                  const __grid_constant__ CUtensorMap tmO, const DgArgs g) {
+  vocab_proj_body<NT, false>(tmW, tmX, tmO, g, nullptr, g.rows);
+}
+
+template <int NT>
+__global__ void __launch_bounds__(DG_THREADS, 1)
+vocab_proj_e4m3_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX,
+                       const __grid_constant__ CUtensorMap tmO, const DgArgs g, const float* w_scale, long long stats_ld) {
+  vocab_proj_body<NT, true>(tmW, tmX, tmO, g, w_scale, stats_ld);
 }
 
 // Shapes both kernels take: one tap, dense rows from row 0, whole k-blocks, no GLU / residual / second output /
@@ -362,14 +443,16 @@ bool dg_supported(const sb_gemm_t* g, int splits) { return wt_supported(g) && sp
 
 // Ring depth, shared memory, tensor maps and launch of either kernel at wgmma N = NT.  The ring is as deep as the
 // opt-in shared memory allows; the products cap it at their K slice and raise it to hold their epilogue's staging
-// tile, which reuses the drained ring.
-template <int NT>
-int wt_launch(const sb_gemm_t* g, DgArgs a, bool proj, cudaStream_t st) {
-  using R = Ring<NT>;
+// tile, which reuses the drained ring.  F8: e4m3 weights with per-feature scales w_scale (the _e4m3 kernels), the
+// ring's stages hold e4m3 weight tiles and two fp16 tiles follow them; stats_ld as in vocab_proj_body.
+template <int NT, bool F8 = false>
+int wt_launch(const sb_gemm_t* g, DgArgs a, bool proj, cudaStream_t st, const float* w_scale = nullptr,
+              long long stats_ld = 0) {
+  using R = Ring<NT, F8>;
   int dev = 0, smem_optin = 0;
   SB_CUDA_OK(cudaGetDevice(&dev));
   SB_CUDA_OK(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  const int extra = proj ? R::STAGING_BYTES : DG_PRODUCTS_SLACK;
+  const int extra = (proj ? R::STAGING_BYTES : DG_PRODUCTS_SLACK) + R::CONV_BYTES;
   const int tiles = (g->n + DG_TM - 1) / DG_TM;
   int stages = (smem_optin - DG_SMEM_MISC - extra) / R::STAGE_BYTES;
   if (stages > DG_MAX_STAGES) stages = DG_MAX_STAGES;
@@ -389,18 +472,24 @@ int wt_launch(const sb_gemm_t* g, DgArgs a, bool proj, cudaStream_t st) {
   a.tiles = tiles;
   const size_t smem = (size_t)stages * R::STAGE_BYTES + extra + DG_SMEM_MISC;
   CUtensorMap tmW, tmX, tmO;
-  int rc = make_tmap(&tmW, g->w, (uint64_t)g->c_in, (uint64_t)g->n, (uint64_t)g->c_in, DG_TM);
+  int rc = make_tmap(&tmW, g->w, (uint64_t)g->c_in, (uint64_t)g->n, (uint64_t)g->c_in, DG_TM, F8 ? 1 : 2);
   if (rc == SB_OK) rc = make_tmap(&tmX, g->a, (uint64_t)g->c_in, (uint64_t)g->m, (uint64_t)g->a_ld, NT);
   if (rc == SB_OK && proj) rc = make_tmap(&tmO, g->out, (uint64_t)g->n, (uint64_t)g->m, (uint64_t)g->out_ld, NT, 4);
   if (rc) return rc;
   static size_t configured[2] = {0, 0};  // per NT, for each kernel
   if (smem > configured[proj]) {
-    const void* k = proj ? (const void*)vocab_proj_kernel<NT> : (const void*)decode_gemm_kernel<NT>;
+    const void* k = F8 ? (proj ? (const void*)vocab_proj_e4m3_kernel<NT> : (const void*)decode_gemm_e4m3_kernel<NT>)
+                       : (proj ? (const void*)vocab_proj_kernel<NT> : (const void*)decode_gemm_kernel<NT>);
     SB_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured[proj] = smem;
   }
-  SB_CUDA_OK(proj ? launch_k(vocab_proj_kernel<NT>, dim3(grid), dim3(DG_THREADS), smem, st, tmW, tmX, tmO, a)
-                  : launch_k(decode_gemm_kernel<NT>, dim3(grid), dim3(DG_THREADS), smem, st, tmW, tmX, a));
+  if constexpr (F8) {
+    SB_CUDA_OK(proj ? launch_k(vocab_proj_e4m3_kernel<NT>, dim3(grid), dim3(DG_THREADS), smem, st, tmW, tmX, tmO, a, w_scale, stats_ld)
+                    : launch_k(decode_gemm_e4m3_kernel<NT>, dim3(grid), dim3(DG_THREADS), smem, st, tmW, tmX, a, w_scale));
+  } else {
+    SB_CUDA_OK(proj ? launch_k(vocab_proj_kernel<NT>, dim3(grid), dim3(DG_THREADS), smem, st, tmW, tmX, tmO, a)
+                    : launch_k(decode_gemm_kernel<NT>, dim3(grid), dim3(DG_THREADS), smem, st, tmW, tmX, a));
+  }
   count_launch();
   return SB_OK;
 }
@@ -411,6 +500,25 @@ int wt_run(const sb_gemm_t* g, const DgArgs& a, bool proj, cudaStream_t st) {
   if (g->m <= 128) return wt_launch<128>(g, a, proj, st);
   if (g->m <= 160) return wt_launch<160>(g, a, proj, st);
   return wt_launch<256>(g, a, proj, st);
+}
+
+int wt_run_e4m3(const sb_gemm_t* g, const DgArgs& a, bool proj, cudaStream_t st, const float* w_scale, long long stats_ld) {
+  if (g->m <= 32) return wt_launch<32, true>(g, a, proj, st, w_scale, stats_ld);
+  if (g->m <= 64) return wt_launch<64, true>(g, a, proj, st, w_scale, stats_ld);
+  if (g->m <= 128) return wt_launch<128, true>(g, a, proj, st, w_scale, stats_ld);
+  if (g->m <= 160) return wt_launch<160, true>(g, a, proj, st, w_scale, stats_ld);
+  return wt_launch<256, true>(g, a, proj, st, w_scale, stats_ld);
+}
+
+// The e4m3 entries' checks: the fp16 kernels' shapes at any row count (run in chunks of DG_MAX_ROWS rows), e4m3 weights
+// whose 64-byte k-blocks TMA can address, and a 4-byte aligned scale array.
+constexpr int DG_MAX_ROWS = 256;
+
+bool e4m3_supported(const sb_gemm_t* g, const float* w_scale) {
+  if (g == nullptr || w_scale == nullptr || ((uintptr_t)w_scale % 4) != 0 || g->m < 1 || g->n < 1) return false;
+  sb_gemm_t c = *g;
+  c.m = 1;
+  return wt_supported(&c);
 }
 
 }  // namespace
@@ -454,4 +562,66 @@ extern "C" int sb_gemm_decode(const sb_gemm_t* g, int32_t splits, float* partial
   a.prefetch = (const char*)g->prefetch;
   a.prefetch_bytes = g->prefetch ? g->prefetch_bytes / 4096 * 4096 : 0;
   return wt_run(g, a, false, (cudaStream_t)stream);
+}
+
+extern "C" int sb_gemm_decode_e4m3(const sb_gemm_t* g, const float* w_scale, int32_t splits, float* partials, int64_t slice_rows,
+                                   sb_stream_t stream) {
+  using namespace sb;
+  SB_REQUIRE(e4m3_supported(g, w_scale) && splits >= 1 && splits <= g->c_in / DG_BK, SB_EINVAL,
+             "sb_gemm_decode_e4m3: needs a 4-byte aligned w_scale, taps 1, c_in %% 64 == 0, 1 <= splits <= c_in / 64, "
+             "16-byte aligned a / w, a_ld %% 8 == 0, no GLU / residual / masking");
+  SB_REQUIRE(partials != nullptr || (splits == 1 && g->out != nullptr && !g->out_f32 && (g->act == SB_ACT_NONE || g->act == SB_ACT_RELU)),
+             SB_EINVAL, "sb_gemm_decode_e4m3: direct mode needs splits == 1, an fp16 output and act in {none, relu}");
+  SB_REQUIRE(partials == nullptr || slice_rows >= g->m, SB_EINVAL, "sb_gemm_decode_e4m3: slice_rows (%lld) < m (%d)",
+             (long long)slice_rows, g->m);
+  SB_REQUIRE(partials != nullptr || ((uintptr_t)g->out % 2) == 0, SB_EINVAL, "sb_gemm_decode_e4m3: misaligned output");
+  SB_REQUIRE(partials == nullptr || ((uintptr_t)partials % 16) == 0, SB_EINVAL, "sb_gemm_decode_e4m3: misaligned partials");
+  // rows are independent: more than 256 run in chunks, each reading the weights again
+  for (int r0 = 0; r0 < g->m; r0 += DG_MAX_ROWS) {
+    sb_gemm_t c = *g;
+    c.m = g->m - r0 < DG_MAX_ROWS ? g->m - r0 : DG_MAX_ROWS;
+    c.a = (const elem_t*)g->a + (long long)r0 * g->a_ld;
+    DgArgs a = {};
+    a.rows = c.m;
+    a.n_out = g->n;
+    a.kb_total = g->c_in / DG_BK;
+    a.splits = splits;
+    a.relu = g->act == SB_ACT_RELU;
+    a.bias = g->bias;
+    a.partials = partials != nullptr ? partials + (long long)r0 * g->n : nullptr;
+    a.slice_rows = slice_rows;
+    a.out = partials != nullptr ? nullptr : (elem_t*)g->out + (long long)r0 * g->out_ld;
+    a.out_ld = g->out_ld;
+    a.prefetch = (const char*)g->prefetch;
+    a.prefetch_bytes = g->prefetch ? g->prefetch_bytes / 4096 * 4096 : 0;
+    const int rc = wt_run_e4m3(&c, a, false, (cudaStream_t)stream, w_scale, 0);
+    if (rc != SB_OK) return rc;
+  }
+  return SB_OK;
+}
+
+extern "C" int sb_vocab_proj_e4m3(const sb_gemm_t* g, const float* w_scale, sb_stream_t stream) {
+  using namespace sb;
+  SB_REQUIRE(e4m3_supported(g, w_scale) && g->act == SB_ACT_NONE && g->out_row0 == 0 && g->out_f32 && g->out != nullptr &&
+                 g->prefetch == nullptr && ((uintptr_t)g->out % 16) == 0 && (g->out_ld % 4) == 0 && g->out_ld >= g->n &&
+                 ((uintptr_t)g->tile_stats % 8) == 0,
+             SB_EINVAL,
+             "sb_vocab_proj_e4m3: needs a 4-byte aligned w_scale, taps 1, c_in %% 64 == 0, 16-byte aligned a / w / out, "
+             "a_ld %% 8 == 0, fp32 output with out_ld %% 4 == 0, act none, no prefetch / GLU / residual / masking");
+  for (int r0 = 0; r0 < g->m; r0 += DG_MAX_ROWS) {
+    sb_gemm_t c = *g;
+    c.m = g->m - r0 < DG_MAX_ROWS ? g->m - r0 : DG_MAX_ROWS;
+    c.a = (const elem_t*)g->a + (long long)r0 * g->a_ld;
+    c.out = (float*)g->out + (long long)r0 * g->out_ld;
+    DgArgs a = {};
+    a.rows = c.m;
+    a.n_out = g->n;
+    a.kb_total = g->c_in / DG_BK;
+    a.bias = g->bias;
+    a.post_scale = g->alpha * g->gamma;
+    a.tile_stats = g->tile_stats != nullptr ? (float2*)g->tile_stats + r0 : nullptr;
+    const int rc = wt_run_e4m3(&c, a, true, (cudaStream_t)stream, w_scale, g->m);
+    if (rc != SB_OK) return rc;
+  }
+  return SB_OK;
 }

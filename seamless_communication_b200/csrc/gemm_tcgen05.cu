@@ -442,18 +442,20 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// 2D tensor (inner = channels, outer = rows), box box_cols x box_rows (box_cols * esize = 128 B), 128B swizzle, OOB -> 0
+// 2D tensor (inner = channels, outer = rows), box box_cols x box_rows (box_cols * esize = 128 B), 128B swizzle, OOB -> 0.
+// esize 1 (e4m3 weight bytes): box 64 x box_rows, unswizzled 64-byte rows.
 int make_tmap(CUtensorMap* tm, const void* base, uint64_t inner, uint64_t rows, uint64_t ld_elems, uint32_t box_rows,
               int esize) {
   EncodeTiledFn fn = get_encode_fn();
   SB_REQUIRE(fn != nullptr, SB_ECUDA, "cuTensorMapEncodeTiled entry point not available");
   cuuint64_t dims[2] = {inner, rows};
   cuuint64_t strides[1] = {ld_elems * (uint64_t)esize};
-  cuuint32_t box[2] = {(cuuint32_t)(128 / esize), box_rows};
+  cuuint32_t box[2] = {(cuuint32_t)(esize == 1 ? 64 : 128 / esize), box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(tm, esize == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
+  CUresult r = fn(tm, esize == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : esize == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
                   const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                  esize == 1 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   SB_REQUIRE(r == CUDA_SUCCESS, SB_ECUDA, "cuTensorMapEncodeTiled failed (%d): inner=%llu rows=%llu ld=%llu esize=%d", (int)r,
              (unsigned long long)inner, (unsigned long long)rows, (unsigned long long)ld_elems, esize);
   return SB_OK;

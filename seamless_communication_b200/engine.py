@@ -71,7 +71,10 @@ def _interleave_glu(w: torch.Tensor) -> torch.Tensor:
 class UnitYEngine:
     decode_fused = False  # bench.py reads it for its decoder-step label: every step is the per-op launch chain
 
-    def __init__(self, cfg: UnitYConfig, state_dict: Dict[str, torch.Tensor], tokenizers, device="cuda"):
+    def __init__(self, cfg: UnitYConfig, state_dict: Dict[str, torch.Tensor], tokenizers, device="cuda",
+                 decoder_weight_dtype=torch.float16):
+        if decoder_weight_dtype not in (torch.float16, torch.float8_e4m3fn):
+            raise ValueError(f"decoder_weight_dtype must be torch.float16 or torch.float8_e4m3fn, got {decoder_weight_dtype}")
         _lib.require_cuda()
         self.cfg = cfg
         self.device = torch.device(device)
@@ -83,7 +86,19 @@ class UnitYEngine:
         self.has_t2u = "t2u_model.decoder_frontend.embed_char.weight" in state_dict
         self.has_t2u_encoder = "t2u_model.encoder.layer_norm.weight" in state_dict
         self.has_encoder = any(k.startswith("speech_encoder.") for k in state_dict)  # a monotonic text decoder has none
+        # FP8 decoder weights (models/fp8_weights.py): the decoder's products and the tied projection read e4m3 weights
+        # with per-feature scales, and every fp16 copy of those weights holds W' = q * scale, so every path computes the
+        # same model
+        self.fp8 = decoder_weight_dtype == torch.float8_e4m3fn
+        q8 = self._quantize_decoder(state_dict) if self.fp8 else None
+        if q8 is not None:
+            from .models.fp8_weights import dequantize_rows
+            state_dict = dict(state_dict)
+            for k, (q, s) in q8.items():
+                state_dict[k] = dequantize_rows(q, s)
         self._pack(state_dict)
+        if q8 is not None:
+            self._pack_e4m3(q8)
         self.pos = sinusoid_table(cfg.max_seq_len, self.M).to(self.device)
         if self.has_t2u:
             self._build_char_tables()
@@ -216,6 +231,28 @@ class UnitYEngine:
                 conv(f"{p}.conv1d.conv1"); conv(f"{p}.conv1d.conv2"); ln(f"{p}.conv1d_layer_norm")
             ln("t2u_model.decoder.layer_norm")
         self.w = w
+
+    def _quantize_decoder(self, sd):
+        """{state-dict name: (q e4m3, scale fp32)} on the device for every weight FP8 mode quantizes."""
+        from .models.fp8_weights import decoder_weight_names, quantize_rows
+        return {k: quantize_rows(sd[k].to(self.device)) for k in decoder_weight_names(sd, self.cfg)}
+
+    def _pack_e4m3(self, q8):
+        """The e4m3 weights and scales of the decoder step beside the fp16 ones: `<name>.q8` (n, K) float8_e4m3fn and
+        `<name>.s` (n,) fp32, q|k|v concatenated as their fp16 copies are."""
+        w = self.w
+
+        def put(key, names):
+            w[key + ".q8"] = torch.cat([q8[n][0] for n in names]).contiguous()
+            w[key + ".s"] = torch.cat([q8[n][1] for n in names]).contiguous()
+
+        put("text_embed", ["text_decoder_frontend.embed.weight"])
+        for i in range(self.cfg.dec_layers):
+            p = f"text_decoder.layers.{i}"
+            put(p + ".self_attn.qkv", [f"{p}.self_attn.{x}_proj.weight" for x in "qkv"])
+            for n in ("self_attn.output_proj", "encoder_decoder_attn.q_proj", "encoder_decoder_attn.output_proj",
+                      "ffn.inner_proj", "ffn.output_proj"):
+                put(f"{p}.{n}", [f"{p}.{n}.weight"])
 
     def _build_char_tables(self):
         """Per-token tables replacing the Python string loops of nar_decoder_frontend.py:130-259."""
@@ -351,24 +388,31 @@ class UnitYEngine:
         self._ln(x, "text_decoder.layers.0.self_attn_layer_norm", out=h)
         S_ATT, S_FFN, S_QKV, SR = st["splits_attn"], st["splits_ffn"], st["splits_qkv"], ops.slice_rows(R)
         pf = self.decode_prefetch  # each GEMM pulls the weights of the GEMM after it into L2 (latency-bound chain)
+        f8 = self.fp8  # e4m3 weights: every product on the e4m3 entries, at any row count
+
+        def splitk(a, name, n, splits, part, nxt):
+            if f8:
+                ops.gemm_splitk_e4m3(a, w[name + ".q8"], w[name + ".s"], n, splits, part,
+                                     prefetch=w[nxt + ".q8"] if pf and nxt else None)
+            else:
+                ops.gemm_splitk(a, w[name + ".w"], n, splits, part, prefetch=w[nxt + ".w"] if pf and nxt else None,
+                                transposed=st["gemm_t"])
+
         for i in range(c.dec_layers):
             p = f"text_decoder.layers.{i}"
             last = i + 1 == c.dec_layers
             nxt = "text_decoder.layer_norm" if last else f"text_decoder.layers.{i + 1}.self_attn_layer_norm"
-            w_next = None if last else w[f"text_decoder.layers.{i + 1}.self_attn.qkv.w"]
+            w_next = None if last else f"text_decoder.layers.{i + 1}.self_attn.qkv"
             # qkv / q projections also run split-K; their partials are reduced (+bias) inside the attention kernels
-            ops.gemm_splitk(h, w[p + ".self_attn.qkv.w"], 3 * M, S_QKV, st["part_qkv"],
-                            prefetch=w[p + ".self_attn.output_proj.w"] if pf else None, transposed=st["gemm_t"])
+            splitk(h, p + ".self_attn.qkv", 3 * M, S_QKV, st["part_qkv"], p + ".self_attn.output_proj")
             check(lib.sb_decode_self_attn(None, st["part_qkv"].data_ptr(), S_QKV, SR, w[p + ".self_attn.qkv.b"].data_ptr(),
                                           st["kc"][i].data_ptr(), st["vc"][i].data_ptr(), st["anc"].data_ptr(), st["ML"],
                                           st["step"].data_ptr(), st["ML"], st["att"].buf.data_ptr(), R, H, stream),
                   "sb_decode_self_attn")
-            ops.gemm_splitk(st["att"], w[p + ".self_attn.output_proj.w"], M, S_ATT, part,
-                            prefetch=w[p + ".encoder_decoder_attn.q_proj.w"] if pf else None, transposed=st["gemm_t"])
+            splitk(st["att"], p + ".self_attn.output_proj", M, S_ATT, part, p + ".encoder_decoder_attn.q_proj")
             ops.splitk_reduce_ln(part, S_ATT, w[p + ".self_attn.output_proj.b"], x, w[p + ".encoder_decoder_attn_layer_norm.w"],
                                  w[p + ".encoder_decoder_attn_layer_norm.b"], h)
-            ops.gemm_splitk(h, w[p + ".encoder_decoder_attn.q_proj.w"], M, S_ATT, part,
-                            prefetch=w[p + ".encoder_decoder_attn.output_proj.w"] if pf else None, transposed=st["gemm_t"])
+            splitk(h, p + ".encoder_decoder_attn.q_proj", M, S_ATT, part, p + ".encoder_decoder_attn.output_proj")
             kv = st["cross_kv"][i].buf
             check(lib.sb_decode_cross_attn(None, part.data_ptr(), S_ATT, SR, w[p + ".encoder_decoder_attn.q_proj.b"].data_ptr(),
                                            kv.data_ptr(), kv[:, M:].data_ptr(), kv.stride(0), ops._p(st["enc_lens"]),
@@ -377,20 +421,26 @@ class UnitYEngine:
             if record and last:  # reads the q partials before the next product overwrites them
                 ops.decode_cross_attn_weights(part, S_ATT, SR, w[p + ".encoder_decoder_attn.q_proj.b"], kv, st["enc_lens"],
                                               st["S_enc"], st["step"], st["attn_hist"], R, st["beam"], H)
-            ops.gemm_splitk(st["att"], w[p + ".encoder_decoder_attn.output_proj.w"], M, S_ATT, part,
-                            prefetch=w[p + ".ffn.inner_proj.w"] if pf else None, transposed=st["gemm_t"])
+            splitk(st["att"], p + ".encoder_decoder_attn.output_proj", M, S_ATT, part, p + ".ffn.inner_proj")
             ops.splitk_reduce_ln(part, S_ATT, w[p + ".encoder_decoder_attn.output_proj.b"], x, w[p + ".ffn_layer_norm.w"],
                                  w[p + ".ffn_layer_norm.b"], h)
-            if st["gemm_t"]:
+            if f8:
+                t = ops.gemm_decode_e4m3(h, w[p + ".ffn.inner_proj.q8"], w[p + ".ffn.inner_proj.s"], c.dec_ffn_dim,
+                                         w[p + ".ffn.inner_proj.b"], act=ACT_RELU, out=st["ffn"],
+                                         prefetch=w[p + ".ffn.output_proj.q8"] if pf else None)
+            elif st["gemm_t"]:
                 t = ops.gemm_decode(h, w[p + ".ffn.inner_proj.w"], c.dec_ffn_dim, w[p + ".ffn.inner_proj.b"], act=ACT_RELU,
                                     out=st["ffn"], prefetch=w[p + ".ffn.output_proj.w"] if pf else None)
             else:
                 t = self._lin(h, p + ".ffn.inner_proj", c.dec_ffn_dim, act=ACT_RELU, out=st["ffn"],
                               prefetch=w[p + ".ffn.output_proj.w"] if pf else None)
-            ops.gemm_splitk(t, w[p + ".ffn.output_proj.w"], M, S_FFN, part, prefetch=w_next if pf else None, transposed=st["gemm_t"])
+            splitk(t, p + ".ffn.output_proj", M, S_FFN, part, w_next)
             ops.splitk_reduce_ln(part, S_FFN, w[p + ".ffn.output_proj.b"], x, w[nxt + ".w"], w[nxt + ".b"], h)
         check(lib.sb_store_step(h.buf.data_ptr(), st["hist"].data_ptr(), st["step"].data_ptr(), R * M * 2, stream), "sb_store_step")
-        ops.gemm(h, w["text_embed"], c.text_vocab, None, out=st["logits"], out_f32=True, tile_stats=st["tile_stats"])
+        if f8:
+            ops.vocab_proj_e4m3(h, w["text_embed.q8"], w["text_embed.s"], c.text_vocab, st["logits"], st["tile_stats"])
+        else:
+            ops.gemm(h, w["text_embed"], c.text_vocab, None, out=st["logits"], out_f32=True, tile_stats=st["tile_stats"])
 
     def _topk(self, st, eos_idx, unk_penalty, bans=None):
         """log-softmax statistics + top-K candidates of every row (st["logits"] / st["tile_stats"] of the last projection).
@@ -461,7 +511,7 @@ class UnitYEngine:
         """Static buffers + captured CUDA graphs of one decoder step, cached per problem shape so that repeated
         predict() calls replay the same graphs (the reference rebuilds its generator per call, translator.py:179-186;
         construction here stays cheap after the first call)."""
-        key = (B, S_enc, ML, beam, P, has_lens, use_graph, self.decode_gemm_t, self.lane)
+        key = (B, S_enc, ML, beam, P, has_lens, use_graph, self.decode_gemm_t and not self.fp8, self.lane)
         st = self._graphs.get(key)
         if st is not None:
             self._graphs.move_to_end(key)

@@ -209,7 +209,7 @@ class UnitYModel:
 
 def load_unity_model(name_or_arch: str, device="cuda", dtype=torch.float16, state_dict: Optional[Dict[str, Tensor]] = None,
                      tokenizers=None, with_t2u: bool = True, seed: int = 0, checkpoint=None, synthetic: bool = False,
-                     **synth_kw) -> UnitYModel:
+                     decoder_weight_dtype=torch.float16, **synth_kw) -> UnitYModel:
     """Resolves an asset-card name to its architecture (reference: models/unity/loader.py:395-402) and builds the engine.
     Weights come from, in this order:
       * `state_dict` - parameters in the reference's fairseq2 naming;
@@ -223,7 +223,12 @@ def load_unity_model(name_or_arch: str, device="cuda", dtype=torch.float16, stat
     A w2v-BERT v1 architecture (`seamlessM4T_large` -> "base") has an autoregressive T2U: it is built when the weights
     hold its unit projection (`t2u_model.final_proj.weight`, or `decoder.output_projection` in fairseq naming) and
     `with_t2u` is set; otherwise the model runs speech-to-text only.  The text encoder is never built (text input is not
-    supported) and its keys are dropped."""
+    supported) and its keys are dropped.
+
+    `decoder_weight_dtype=torch.float8_e4m3fn` runs the text decoder's beam search (and the AR T2U's unit search) on
+    weight-only FP8: its six products per layer and the tied projection read e4m3 weights with one power-of-two scale
+    per output feature.  The model computed is exactly the fp16 model on `dequantize_decoder_weights(state_dict, cfg)`
+    (models/fp8_weights.py).  The default, torch.float16, runs the weights as given."""
     arch = cfgmod.MODEL_CARDS.get(name_or_arch, name_or_arch)
     if arch not in cfgmod.UNITY_ARCHS:
         raise ValueError(f"unknown model card / architecture '{name_or_arch}'")
@@ -260,7 +265,9 @@ def load_unity_model(name_or_arch: str, device="cuda", dtype=torch.float16, stat
         ar = {k: v for k, v in state_dict.items() if k.startswith("t2u_model.")}
         state_dict = {k: v for k, v in state_dict.items() if k not in ar or k.startswith("t2u_model.encoder.")}
         if "t2u_model.final_proj.weight" in ar:
-            unit_engine = UnitYEngine(t2u_decoder_config(cfg), t2u_decoder_state_dict(ar), (None, None), device=device)
+            unit_engine = UnitYEngine(t2u_decoder_config(cfg), t2u_decoder_state_dict(ar), (None, None), device=device,
+                                      decoder_weight_dtype=decoder_weight_dtype)
         else:  # no AR T2U (an S2TT-only checkpoint): its encoder is not built either
             state_dict = {k: v for k, v in state_dict.items() if not k.startswith("t2u_model.")}
-    return UnitYModel(cfg, UnitYEngine(cfg, state_dict, tokenizers, device=device), unit_engine)
+    return UnitYModel(cfg, UnitYEngine(cfg, state_dict, tokenizers, device=device, decoder_weight_dtype=decoder_weight_dtype),
+                      unit_engine)

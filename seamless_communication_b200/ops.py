@@ -191,6 +191,55 @@ def gemm_decode(a: Seq, w: torch.Tensor, n: int, bias, act=ACT_NONE, out: Option
     return out
 
 
+def _desc_e4m3(a: Seq, w: torch.Tensor, n: int) -> GemmDesc:
+    if w.dtype != torch.float8_e4m3fn:
+        raise TypeError(f"the e4m3 entries take float8_e4m3fn weights, got {w.dtype}")
+    assert a.PH == 0 and a.Tp == a.T
+    d = GemmDesc()
+    d.a, d.a_rows, d.a_ld, d.c_in, d.taps, d.dil, d.a_row0 = a.buf.data_ptr(), a.B * a.T, a.buf.stride(0), a.C, 1, 1, 0
+    d.w, d.n, d.m = w.data_ptr(), n, a.B * a.T
+    return d
+
+
+def gemm_splitk_e4m3(a: Seq, w: torch.Tensor, w_scale: torch.Tensor, n: int, splits: int, partials: torch.Tensor,
+                     prefetch: Optional[torch.Tensor] = None) -> None:
+    """gemm_splitk(transposed=True) on e4m3 weights w (n, K) with fp32 per-feature scales (sb_gemm_decode_e4m3): the
+    partials of the fp16 weights w * w_scale, at any row count."""
+    d = _desc_e4m3(a, w, n)
+    if prefetch is not None:
+        d.prefetch, d.prefetch_bytes = prefetch.data_ptr(), prefetch.numel() * prefetch.element_size()
+    check(_lib.load().sb_gemm_decode_e4m3(C.byref(d), w_scale.data_ptr(), splits, partials.data_ptr(), slice_rows(a.B * a.T),
+                                          _stream()), "sb_gemm_decode_e4m3")
+
+
+def gemm_decode_e4m3(a: Seq, w: torch.Tensor, w_scale: torch.Tensor, n: int, bias, act=ACT_NONE, out: Optional[Seq] = None,
+                     prefetch: Optional[torch.Tensor] = None) -> Seq:
+    """gemm_decode on e4m3 weights with per-feature scales (sb_gemm_decode_e4m3, direct mode), at any row count."""
+    if out is None:
+        out = Seq(a.B, a.T, n)
+    d = _desc_e4m3(a, w, n)
+    d.bias, d.act = _p(bias), act
+    d.out, d.out_ld = out.buf.data_ptr(), out.buf.stride(0)
+    if prefetch is not None:
+        d.prefetch, d.prefetch_bytes = prefetch.data_ptr(), prefetch.numel() * prefetch.element_size()
+    check(_lib.load().sb_gemm_decode_e4m3(C.byref(d), w_scale.data_ptr(), 1, None, 0, _stream()), "sb_gemm_decode_e4m3")
+    return out
+
+
+def vocab_proj_e4m3(a: Seq, w: torch.Tensor, w_scale: torch.Tensor, n: int, out: Seq, tile_stats: Optional[torch.Tensor] = None,
+                    bias=None, alpha=1.0) -> Seq:
+    """The tied projection on e4m3 weights (sb_vocab_proj_e4m3): fp32 out = (a . (w * w_scale)^T + bias) * alpha, with the
+    per-(128-column tile, row) log-softmax statistics when tile_stats is given - what gemm(out_f32=True, tile_stats=...)
+    writes for the fp16 weights w * w_scale."""
+    d = _desc_e4m3(a, w, n)
+    d.bias, d.alpha, d.gamma = _p(bias), alpha, 1.0
+    d.out, d.out_ld, d.out_f32 = out.buf.data_ptr(), out.buf.stride(0), 1
+    if tile_stats is not None:
+        d.tile_stats = tile_stats.data_ptr()
+    check(_lib.load().sb_vocab_proj_e4m3(C.byref(d), w_scale.data_ptr(), _stream()), "sb_vocab_proj_e4m3")
+    return out
+
+
 def splitk_reduce_ln(partials: torch.Tensor, splits: int, bias, x: Seq, ln_w, ln_b, h: Seq) -> None:
     lib = _lib.load()
     check(lib.sb_splitk_reduce_ln(partials.data_ptr(), splits, x.B * x.T, slice_rows(x.B * x.T), x.C, _p(bias), x.buf.data_ptr(), ln_w.data_ptr(),
