@@ -14,7 +14,11 @@ Named architectures:
     encoder, same 600m / dense_1b dims), with ``tiny_v1`` / ``small_v1`` test
     copies.  Their T2U is the autoregressive one (t2u_builder.py:141-160
     `_base_t2u`): a pre-LN Transformer encoder and an NLLB-type decoder over the
-    unit vocabulary, sized by the same ``t2u_*`` / ``unit_*`` fields.
+    unit vocabulary, sized by the same ``t2u_*`` / ``unit_*`` fields;
+  * ``medium``   - seamlessM4T_medium (builder.py:137-162 `_medium`,
+    t2u_builder.py:163-183 `_medium_t2u`): the v1 stack with w2v-BERT "300m"
+    (12 Conformer layers), NLLB "dense_600m" (12 decoder layers, FFN 4096) over
+    NLLB-200's 256 206 tokens and a 4 + 4 layer AR T2U.
 """
 from __future__ import annotations
 
@@ -29,6 +33,17 @@ NLLB100_LANGS: Tuple[str, ...] = tuple(
     "fin fra fuv gaz gle glg guj heb hin hrv hun hye ibo ind isl ita jav jpn kan kat kaz khk khm kir kor lao "
     "lit lug luo lvs mai mal mar mkd mlt mni mya nld nno nob npi nya ory pan pbt pes pol por ron rus sat slk "
     "slv sna snd som spa srp swe swh tam tel tgk tgl tha tur ukr urd uzn vie yor yue zsm zul".split()
+)
+# cards/unity_nllb-200.yaml `langs` (seamlessM4T_medium), in card order: the `__lang__` ids of the tokenizer follow it
+NLLB200_LANGS: Tuple[str, ...] = tuple(
+    "ace ace_Latn acm acq aeb afr ajp aka amh apc arb ars ary arz asm ast awa ayr azb azj bak bam ban bel bem ben bho "
+    "bjn bjn_Latn bod bos bug bul cat ceb ces cjk ckb crh cym dan deu dik dyu dzo ell eng epo est eus ewe fao pes fij "
+    "fin fon fra fur fuv gla gle glg grn guj hat hau heb hin hne hrv hun hye ibo ilo ind isl ita jav jpn kab kac kam "
+    "kan kas kas_Deva kat knc knc_Latn kaz kbp kea khm kik kin kir kmb kon kor kmr lao lvs lij lim lin lit lmo ltg "
+    "ltz lua lug luo lus mag mai mal mar min mkd plt mlt mni khk mos mri zsm mya nld nno nob npi nso nus nya oci gaz "
+    "ory pag pan pap pol por prs pbt quy ron run rus sag san sat scn shn sin slk slv smo sna snd som sot spa als srd "
+    "srp ssw sun swe swh szl tam tat tel tgk tgl tha tir taq taq_Tfng tpi tsn tso tuk tum tur twi tzm uig ukr umb urd "
+    "uzn vec vie war wol xho ydd yor yue cmn cmn_Hant zul".split()
 )
 UNIT_LANGS_V2: Tuple[str, ...] = tuple(
     "arb ben cat ces cmn cym dan deu eng est fin fra hin ind ita jpn kan kor mlt nld pes pol por ron rus slk "
@@ -297,6 +312,14 @@ def base() -> UnitYConfig:
     return UnitYConfig(name="base", encoder_variant="v1")
 
 
+def medium() -> UnitYConfig:
+    """seamlessM4T_medium: the v1 stack of `base` with w2v-BERT "300m" (12 Conformer layers), NLLB "dense_600m" (12
+    decoder layers, FFN 4096; both recalled, DESIGN.md section 17), NLLB-200's vocabulary and languages, and the AR T2U
+    `_medium_t2u` (4 + 4 layers, FFN 8192, the same 10 082 units).  The adaptor and `max_seq_len` are base's."""
+    return UnitYConfig(name="medium", encoder_variant="v1", enc_layers=12, dec_layers=12, dec_ffn_dim=4096,
+                       text_vocab=256206, t2u_enc_layers=4, t2u_dec_layers=4, langs=NLLB200_LANGS)
+
+
 def tiny_v1() -> UnitYConfig:
     c = tiny_v2()
     c.name, c.encoder_variant = "tiny_v1", "v1"
@@ -326,13 +349,13 @@ def tiny_vocoder() -> VocoderConfig:
 
 
 UNITY_ARCHS = {"base_v2": base_v2, "tiny_v2": tiny_v2, "small_v2": small_v2, "base": base, "tiny_v1": tiny_v1,
-               "small_v1": small_v1}
+               "small_v1": small_v1, "medium": medium}
 VOCODER_ARCHS = {"base": base_vocoder, "tiny": tiny_vocoder}
 
 # asset-card names the reference resolves through fairseq2's asset store
 # (cards/seamlessM4T_v2_large.yaml: model_arch base_v2; cards/vocoder_v2.yaml and vocoder_36langs.yaml: base)
 MODEL_CARDS = {"seamlessM4T_v2_large": "base_v2", "seamlessM4T_v2_tiny": "tiny_v2", "seamlessM4T_v2_small": "small_v2",
-               "seamlessM4T_large": "base"}
+               "seamlessM4T_large": "base", "seamlessM4T_medium": "medium"}
 VOCODER_CARDS = {"vocoder_v2": "base", "vocoder_v2_tiny": "tiny", "vocoder_36langs": "base"}
 
 # cards/mintox.yaml (the ETOX word lists of MinTox, toxicity/etox_bad_word_checker.py): word files named after one of

@@ -207,6 +207,29 @@ class UnitYModel:
         return [self.engine] + ([t2u.unit_engine] if isinstance(t2u, UnitYT2UModel) else [])
 
 
+def _layer_count(sd: Dict[str, Tensor], prefix: str) -> Optional[int]:
+    """1 + the largest layer index under `prefix` ("...layers."), or None when the state dict has no such layer."""
+    idx = [int(k[len(prefix):].split(".", 1)[0]) for k in sd if k.startswith(prefix)]
+    return max(idx) + 1 if idx else None
+
+
+def check_state_dict(sd: Dict[str, Tensor], cfg) -> None:
+    """Refuse weights of another architecture before anything is built: the layer counts of the speech encoder, the
+    text decoder and the T2U encoder and decoder (each where the state dict has it), the text decoder's FFN width and the
+    vocabulary size of its tied table must be the config's.  Raises ValueError naming the first mismatch."""
+    checks = [("speech encoder layers", _layer_count(sd, "speech_encoder.inner.layers."), cfg.enc_layers),
+              ("text decoder layers", _layer_count(sd, "text_decoder.layers."), cfg.dec_layers)]
+    ffn = sd.get("text_decoder.layers.0.ffn.inner_proj.weight")
+    checks.append(("text decoder FFN width", None if ffn is None else ffn.shape[0], cfg.dec_ffn_dim))
+    emb = sd.get("final_proj.weight", sd.get("text_decoder_frontend.embed.weight"))
+    checks.append(("text vocabulary size", None if emb is None else emb.shape[0], cfg.text_vocab))
+    checks += [("T2U encoder layers", _layer_count(sd, "t2u_model.encoder.layers."), cfg.t2u_enc_layers),
+               ("T2U decoder layers", _layer_count(sd, "t2u_model.decoder.layers."), cfg.t2u_dec_layers)]
+    for what, got, want in checks:
+        if got is not None and got != want:
+            raise ValueError(f"the weights do not fit architecture '{cfg.name}': {what} {got}, the architecture has {want}")
+
+
 def load_unity_model(name_or_arch: str, device="cuda", dtype=torch.float16, state_dict: Optional[Dict[str, Tensor]] = None,
                      tokenizers=None, with_t2u: bool = True, seed: int = 0, checkpoint=None, synthetic: bool = False,
                      decoder_weight_dtype=torch.float16, **synth_kw) -> UnitYModel:
@@ -224,6 +247,9 @@ def load_unity_model(name_or_arch: str, device="cuda", dtype=torch.float16, stat
     hold its unit projection (`t2u_model.final_proj.weight`, or `decoder.output_projection` in fairseq naming) and
     `with_t2u` is set; otherwise the model runs speech-to-text only.  The text encoder is never built (text input is not
     supported) and its keys are dropped.
+
+    The weights of `seamlessM4T_medium` are checked against the architecture first (`check_state_dict`): layer counts,
+    the decoder's FFN width and the vocabulary size.  A mismatch raises ValueError.
 
     `decoder_weight_dtype=torch.float8_e4m3fn` runs the text decoder's beam search (and the AR T2U's unit search) on
     weight-only FP8: its six products per layer and the tied projection read e4m3 weights with one power-of-two scale
@@ -260,6 +286,8 @@ def load_unity_model(name_or_arch: str, device="cuda", dtype=torch.float16, stat
         drop = ("text_encoder.", "text_encoder_frontend.") if v1 else ()
         drop += () if with_t2u else ("t2u_model.",)
         state_dict = {k: v for k, v in state_dict.items() if not k.startswith(drop)}
+    if arch == "medium":
+        check_state_dict(state_dict, cfg)
     unit_engine = None
     if v1:
         ar = {k: v for k, v in state_dict.items() if k.startswith("t2u_model.")}
